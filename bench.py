@@ -2,9 +2,10 @@
 """Benchmark of the geometric propagate hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+                    [--dump-outputs DIR]
 
 Workload (N=1, and per rank for N>1 -- weak scaling): BASELINE.json configs[1],
-"Double-Gauss 12-surface, 1e7 rays, 3 wavelengths, FP64, 1xB200": one STEP is
+"Double-Gauss 12-surface, 1e7 rays, 3 wavelengths, FP64, 1xH100": one STEP is
 one pass of the hot path over the three wavelength bundles (3 launches of the
 trace kernel, 1e7 aimed rays x 12 surfaces each, clip=True, full trace
 y,u,i,t stored).  Metric: ray-surface intersections per second.
@@ -24,13 +25,22 @@ y,u,i,t stored).  Metric: ray-surface intersections per second.
             on all host cores: the whole workload ray-sharded over the cores;
             numpy port as fallback
   headline  (N=1, when the HBM is free) the north-star point: zoom S=20,
-            1e8 rays, FP64, full trace resident, one launch
+            3e7 rays, FP64, full trace resident (49 GB), one launch
   c3        (N=1) BASELINE config C3: Cooke + aspheres, 1e8 rays, FP32
   multi_gpu (N>1) C4: every rank traces 1.25e8 rays generated in HBM and the
             SAME kernel stores y[-1] into the gather buffers of all ranks over
             NVLink (rtx_trace_gather); C5: the 25 zoom bundles split by rays
             so that every rank carries 25/N bundles' worth
   parity_ok samples of the timed results checked against the oracle (asserted)
+
+`--dump-outputs DIR` (rank 0): after the timed steps, the trace arrays the
+last step computed -- DIR/{y,u,i,t}_l<k>.npy, float64, wavelength k, shape
+(S, 16384, 3) / (S, 16384) -- for every (N // 16384)-th launch ray (all of
+them when N <= 16384).  A vignetted ray is NaN from its clipping surface on;
+the files hold 0 there instead and DIR/vignetted_l<k>.npy, shape (S, 16384),
+is 1.0 where any of y,u,i,t of that ray and surface was not finite, so every
+file is finite and nothing is lost.  The launch rays depend only on the
+arguments, so two builds can be compared output for output.
 
 `--impl reference` times the reference's own CPU path -- GeometricTrace.
 rays_given + propagate of quartiq/rayopt -- on the same workload, ray-sharded
@@ -140,17 +150,14 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
 
 
 def cpu_reference(steps, warmup):
     """The reference's CPU path on all host cores, in its own process
     (oracle/cpu_bench.py: no fork out of a CUDA process, no inherited NUMA
     binding): every step is the WHOLE C2 workload -- 1e7 rays per wavelength,
-    ray-sharded over os.cpu_count() processes (78 125 rays per process on a
-    128-thread host; with 4e5 rays per process the same host measured 3.0e7
-    ray-surfaces/s, profiles/r2a_bench.json, so the natural sharding is also
-    the reference's better case).  Returns cpu_bench's dict."""
+    ray-sharded over os.cpu_count() processes.  Returns cpu_bench's dict."""
     cmd = [sys.executable, os.path.join(ROOT, "oracle", "cpu_bench.py"), "--system", SYSTEM,
            "--field", str(FIELD[0]), str(FIELD[1]), "--rays-total", str(N_RAYS),
            "--steps", str(steps), "--warmup", str(warmup)]
@@ -199,13 +206,14 @@ def check_sample(got, want, what, tol=1e-10):
 
 
 # --------------------------------------------------------------------------
-def leg_headline(eng, exact):
-    """north-star point on one GPU: zoom S=20, ~1e8 rays (hexapolar grid
-    generated in HBM), FP64, full trace resident, ONE launch per trace"""
+def leg_headline(eng, exact, NR=30_000_000):
+    """north-star point on one GPU: zoom S=20, ~3e7 rays (hexapolar grid
+    generated in HBM), FP64, full trace resident (49 GB of an 80 GB H100), ONE
+    launch per trace"""
     from rayopt_b200.rays import aim_infinite, hexapolar_xy
     ent = load_system("zoom")
     S, table, aim = ent["S"], ent["tables"][0], ent["aim"][0][FIELD_INDEX]
-    rings = int(np.sqrt(1e8/3. - 1/12.) - 1/2.)
+    rings = int(np.sqrt(NR/3. - 1/12.) - 1/2.)
     N = 1 + 3*rings*(rings + 1)
     ld = (N + 63)//64*64
     need = N*48 + S*ld*80
@@ -213,7 +221,7 @@ def leg_headline(eng, exact):
     if free < need + (2 << 30):
         return {"skipped": "needs %.1f GB of HBM, %.1f GB free" % (need/1e9, free/1e9)}
     y0, u0 = eng.aim_infinite_device(aim["field"], aim["z"], aim["p"], ent["object_angle"],
-                                     nrays=10**8)
+                                     nrays=NR)
     out = [eng.empty((S, ld, 3)) for _ in range(3)] + [eng.empty((S, ld))]
     ms = []
     for _ in range(4):
@@ -465,6 +473,32 @@ def leg_c5(eng, dist, torch, exact, NR=10_000_000):
             "parity_ok": bool(ok.item() == 1.0), "parity_this_rank": par}
 
 
+def dump_outputs(eng, dev, S, N, out_dir, K=16384):
+    """y,u,i,t of every bundle at rays 0, d, 2d, ... (d = N // K): K rays,
+    S surfaces, float64, non-finite entries as 0 plus the per-surface
+    vignetting mask -- 52 MB for the default workload"""
+    from rayopt_b200._lib import check, ptr
+    os.makedirs(out_dir, exist_ok=True)
+    K = min(K, N)
+    step = N//K
+    idx = np.arange(K)*step
+    for li, d in enumerate(dev):
+        out = {k.lower(): np.stack([eng.download_rays(d[k].rows(s), idx) for s in range(S)])
+               for k in "YUI"}
+        t = np.empty((S, K))
+        for s in range(S):        # T rows hold one value per ray: one strided copy per row
+            check(eng.lib.rtx_memcpy2d_d2h(eng.ctx, ptr(t[s]), 8, d["T"].rows(s).ptr, step*8, 8, K))
+        eng.sync()
+        out["t"] = t
+        bad = ~np.isfinite(t)
+        for k in "yui":
+            bad |= ~np.isfinite(out[k]).all(axis=2)
+        for k, a in out.items():
+            np.save(os.path.join(out_dir, "%s_l%d.npy" % (k, li)),
+                    np.where(np.isfinite(a), a, 0.0))
+        np.save(os.path.join(out_dir, "vignetted_l%d.npy" % li), bad.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -479,6 +513,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-headline", action="store_true")
     ap.add_argument("--no-multi", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write a fixed sample of the last timed step's y,u,i,t as .npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -568,6 +604,8 @@ def main():
     ms = eng.timer_stop()
     t_wall1 = time.time()
     launches = eng.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, dev, S, N, args.dump_outputs)
     for _ in range(3):              # samples right after the region are still under load
         step()
     barrier()
@@ -589,10 +627,9 @@ def main():
     alg_bytes = N*(6*w + 10*w*S)
     achieved = alg_bytes/(k_ms*1e-3)/1e9
     peak, peak_src = peaks()
-    # DRAM traffic per launch is NOT measurable from inside the process (it
-    # needs ncu): the number below is carried over from the committed ncu
-    # capture of this kernel at this size and labelled as such
-    traffic = 10_017_400_000 if (N == N_RAYS and not args.direct) else None
+    # DRAM traffic per launch is not measurable from inside the process (it
+    # needs a hardware-counter profiler): reported as not measured
+    traffic = None
 
     # ---- parity of the timed device-resident results (sample vs the oracle)
     idx = np.arange(0, N, max(1, N//2000))[:2000]
@@ -772,13 +809,11 @@ def main():
                        "numa_node": node,
                        "rays": "aimed bundles generated in HBM (rtx_aim_rays, random disc, seed per "
                                "rank and wavelength)",
-                       "l2": "outputs %.1f GB per launch >> 126 MB L2 (no flush needed)"
+                       "l2": "outputs %.1f GB per launch >> 50 MB L2 (no flush needed)"
                              % (alg_bytes/1e9)},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": achieved/peak, "traffic": traffic,
-                         "traffic_source": "from profile, not measured in this run: ncu "
-                                           "dram__bytes_read.sum+dram__bytes_write.sum per launch of "
-                                           "this kernel at this size, profiles/r2c_dram_bytes_full_size.csv",
+                         "traffic_source": "not measured",
                          "peak_source": peak_src,
                          "kernel": "rtx::trace_kernel<double>", "kernel_ms": k_ms,
                          "algorithmic_bytes_per_launch": alg_bytes},

@@ -1,5 +1,5 @@
 /*
- * rtx.h -- C ABI of the B200-native sequential geometric ray-trace engine.
+ * rtx.h -- C ABI of the H100-native (sm_90a) sequential geometric ray-trace engine.
  *
  * This is the drop-in boundary for ONE hot path of quartiq/rayopt: the
  * per-surface  transfer -> intercept -> clip -> refract  loop

@@ -103,7 +103,12 @@ def intercept_newton(rec, y, u):
             zero = active & (fder == 0)                   # RuntimeError -> NaN
             active &= ~zero
             p = p0 - fval/fder
-            conv = active & (np.abs(p - p0) <= NEWTON_TOL)  # np.isclose rtol=0
+            tol = NEWTON_TOL
+            if p.dtype == np.float32:
+                # 1e-7 is below float32 resolution for |p| > 1: a few ulp of the
+                # iterate instead, the FP32 engine's rule (rtx_device.cuh)
+                tol = np.maximum(np.float32(NEWTON_TOL), np.float32(4*2.0**-23)*np.abs(p))
+            conv = active & (np.abs(p - p0) <= tol)        # np.isclose rtol=0
             conv |= active & (p == p0)                    # equal infinities
             out[conv] = p[conv]
             active &= ~conv

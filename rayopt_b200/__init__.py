@@ -1,8 +1,8 @@
-"""rayopt_b200 -- B200-native engine for rayopt's geometric propagate loop.
+"""rayopt_b200 -- H100-native engine for rayopt's geometric propagate loop.
 
 Hot path only: ``GeometricTrace.propagate`` / ``System.propagate``
 (rayopt/geometric_trace.py:72-80, rayopt/system.py:459-464) as one hand-written
-CUDA (sm_100a) launch behind a C ABI (include/rtx.h).  No PyTorch, no CPU
+CUDA (sm_90a) launch behind a C ABI (include/rtx.h).  No PyTorch, no CPU
 fallback: importing works anywhere, tracing needs librtx.so and a GPU.
 """
 from .surface_table import (SURFACE_DTYPE, PackedSystem, pack_system,  # noqa: F401

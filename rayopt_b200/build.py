@@ -1,8 +1,8 @@
-"""In-tree build of the CUDA library (nvcc, sm_100a only).
+"""In-tree build of the CUDA library (nvcc, sm_90a only: H100).
 
     python -m rayopt_b200.build          # rebuild if sources are newer
 
-The .so is git-ignored but travels to the GPU box with the repo snapshot.
+The .so is a git-ignored build product next to this file.
 """
 import os
 import shutil
@@ -16,7 +16,7 @@ SOURCES = ["rtx.cu"]
 HEADERS = ["rtx_device.cuh", os.path.join("..", "..", "include", "rtx.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]

@@ -1,6 +1,6 @@
 // rtx.cu -- C ABI of the ray-trace engine (include/rtx.h): context, memory,
 // the table conversion and the kernel launches.  Build:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared \
 //        -Xcompiler -fPIC -o librtx.so rtx.cu
 #include "../../include/rtx.h"
 #include "rtx_device.cuh"
@@ -76,7 +76,7 @@ struct rtx_ctx {
     size_t small_bytes = 0;
     int64_t launches = 0;
     int max_smem_optin = 0;
-    // kernel configuration (defaults = measured best, profiles/r1_sweep*.txt)
+    // kernel configuration (defaults; trace_device picks per call)
     int default_rpt = 2;      // rays per thread
     int store = 2;            // STORE_WARP / STORE_CTA
     int warps = 16;           // warps per CTA
@@ -369,21 +369,18 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
     bool heavy = false;
     const bool explicit_rpt = (flags & (RTX_RPT1 | RTX_RPT2)) != 0;
     if (!ctx->tuned && !explicit_rpt) {
-        // measured best configurations (profiles/r1_sweep8_defaults.txt,
-        // r2b_sweep_newton_rewrite.txt; fractions of the measured HBM copy peak):
-        //  FP64: 2 rays/thread x 16 warps, per-CTA bulk stores (24 KB runs)      0.93-0.95
+        // configurations by workload (scripts/sweep.py compares them):
+        //  FP64: 2 rays/thread x 16 warps, per-CTA bulk stores (24 KB runs)
         //  FP32: 4 rays/thread x 16 warps (2048-ray tiles, 24 KB runs again):
-        //        half the per-thread overhead instructions of 2 rays/thread     0.92-0.94
+        //        half the per-thread overhead instructions of 2 rays/thread
         //  systems with >= 25 % Newton (aspheric) surfaces are bound by issue
         //  slots / the FP64 pipe, not by HBM: free-running 16-warp CTAs with
         //  per-warp stores (no lockstep barrier behind the long, divergent
-        //  Newton chains) -- FP64 0.88, FP32 (4 rays per thread) 0.88
-        //  (profiles/r2l_sweep_heavy_configs.txt)
+        //  Newton chains)
         int newton = 0;
         for (int i = 0; i < S; ++i) newton += surf && surf[i].n_asph >= 0;
         // ... and so is a keep-LAST trace (one stored row: the stores are no
-        // limit): free-running CTAs, 1e7 rays x 12 surfaces 0.94 -> 0.84 ms
-        // (profiles/r2p_keep_last_configs.txt)
+        // limit): free-running CTAs
         // (a fused gather keeps the per-CTA 24 KB runs for its NVLink stores)
         heavy = newton * 4 >= S || (keep == RTX_KEEP_LAST && !(peers && peers->n > 0));
         if (sizeof(T) == 4) {
@@ -398,9 +395,7 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
                 nbuf = 1;
             }
         } else if (heavy) {
-            // free-running 16-warp CTAs with per-warp stores (fast 0.88, RTX_EXACT
-            // 0.80; 8-warp CTAs: 0.855 with per-CTA stores / 0.77 exact on the
-            // same box, profiles/r2l_sweep_heavy_configs.txt)
+            // free-running 16-warp CTAs with per-warp stores
             rpt = 2;
             store = STORE_WARP;
             nbuf = 2;
@@ -408,8 +403,7 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
         }
     }
     if (N <= 150 * 1000 && !ctx->tuned) {
-        // small bundles: 256-ray warp tiles spread over all SMs (5e4 rays:
-        // 0.35 vs 0.24 with 1024-ray tiles, profiles/r2n_midsize_configs.txt)
+        // small bundles: 256-ray warp tiles spread over all SMs
         rpt = 1;
         store = STORE_WARP;
         warps = 8;
@@ -417,7 +411,6 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
     } else if (N <= 1500 * 1000 && !ctx->tuned && !explicit_rpt && !heavy && sizeof(T) == 8) {
         // mid-size FP64 bundles (what an analysis traces): 512-ray tiles, two
         // resident CTAs per SM -- twice the tiles to balance over the SMs
-        // (3e5 rays 0.78 -> 0.88, 1e6 rays 0.81 -> 0.88)
         rpt = 1;
         store = STORE_CTA;
         warps = 16;
@@ -425,7 +418,6 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
     } else if (N > 500 * 1000 && N <= 2500 * 1000 && !ctx->tuned && !explicit_rpt && !heavy &&
                sizeof(T) == 4) {
         // mid-size FP32 bundles: 512-ray tiles, three resident CTAs per SM
-        // (1e6 rays 0.72 -> 0.92, 2e6 rays 0.81 -> 0.83)
         rpt = 2;
         store = STORE_CTA;
         warps = 8;
@@ -753,7 +745,7 @@ int rtx_init(int device, rtx_ctx** out) {
         rtx_free(ctx);
         return rc;
     }
-    // tuning knobs (experiments; the defaults above are the measured best)
+    // tuning knobs (experiments; they override the per-call choice above)
     if (const char* e = getenv("RTX_RPT")) {
         int v = atoi(e);
         if (v == 1 || v == 2 || v == 4) ctx->default_rpt = v;

@@ -2,7 +2,7 @@
 """Opcode histogram of every kernel in librtx.so (cuobjdump -sass): the
 evidence that the TMA bulk-copy path (UBLKCP / SYNCS / UTMACMDFLUSH), the
 mbarrier waits and the FP64 / FP32 pipes are what the kernels use.
-    python scripts/sass_opcodes.py > profiles/r2_sass_opcodes.txt"""
+    python scripts/sass_opcodes.py > sass_opcodes.txt"""
 import collections, os, re, subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "rayopt_b200", "librtx.so")

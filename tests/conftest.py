@@ -14,7 +14,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), GOLDEN):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def _cuda_device_count():

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz and systems.json FROM THE LIVE REFERENCE.
 
-Run in the build container only (needs /root/reference, read-only):
+Needs the reference tree (oracle/ref_shim.py: $RAYOPT_REFERENCE or oracle/_ref):
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py                  # *.npz, systems.json
+    python tests/golden/make_golden.py --vs-reference   # vs_reference/*.npz
 
 For every case the reference's own System / GeometricTrace (imported through
 oracle/ref_shim.py) produces launch rays and the full trace; the case file
@@ -263,5 +264,37 @@ def main():
     save("cooke_single_ray", s, g, False)
 
 
+VS_REFERENCE = [("cooke", 20000, False), ("double_gauss", 20000, True),
+                ("zoom", 10000, True), ("cooke_asph", 400, True), ("mirror", 5000, False),
+                ("singlet", 5000, True)]
+
+
+def vs_reference(keep=32):
+    """vs_reference/<system>.npz: the reference's packed table, launch rays and
+    full trace for the first two wavelengths of each fixture system (field
+    (0, .7), n pupil points uniform in the disc), for a seeded sample of `keep`
+    of those rays (tests/test_oracle_vs_reference.py)"""
+    os.makedirs(os.path.join(HERE, "vs_reference"), exist_ok=True)
+    for name, n, clip in VS_REFERENCE:
+        s = build(systems_yaml.SYSTEMS[name])
+        out = {"clip": np.array(bool(clip)), "n_rays": np.array(n)}
+        for j, l in enumerate(s.wavelengths[:2]):
+            g, z, p = trace_aimed(s, (0, .7), l, disc(n, 1), clip)
+            table, nn, rot0 = pack_system(s, l)
+            assert np.array_equal(nn, g.n[1:])
+            idx = np.sort(np.random.default_rng(j).choice(n, min(n, keep), replace=False))
+            out.update({"table%d" % j: table, "n%d" % j: nn,
+                        "rot0%d" % j: np.zeros((0, 3)) if rot0 is None else rot0,
+                        "idx%d" % j: idx, "y0%d" % j: g.y[0][idx], "u0%d" % j: g.u[0][idx],
+                        "Y%d" % j: g.y[1:, idx], "U%d" % j: g.u[1:, idx],
+                        "I%d" % j: g.i[1:, idx], "T%d" % j: g.t[1:, idx]})
+        path = os.path.join(HERE, "vs_reference", name + ".npz")
+        np.savez_compressed(path, **out)
+        print("%-14s %6.1f kB" % (name, os.path.getsize(path)/1e3))
+
+
 if __name__ == "__main__":
-    main()
+    if "--vs-reference" in sys.argv:
+        vs_reference()
+    else:
+        main()

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""North-star headline point: zoom fixture, 1e8 rays x 20 surfaces, FP64, full
-trace device-resident on ONE B200 (164.8 GB of algorithmic traffic per
-launch, 160 GB of results in HBM).  The 1e8-ray bundle is ten copies of a
+"""North-star headline point: zoom fixture, 3e7 rays x 20 surfaces, FP64, full
+trace device-resident on ONE 80 GB H100 (49.4 GB of algorithmic traffic per
+launch, 48 GB of results in HBM).  The 3e7-ray bundle is three copies of a
 1e7-ray aimed bundle (synthetic; distinct seeds per copy would only change
 the host generation time)."""
 import json, os, statistics, sys
@@ -12,7 +12,7 @@ import bench, np_oracle
 from rayopt_b200.engine import Engine
 from rayopt_b200._lib import check, ptr
 
-N1, COPIES = 10_000_000, int(os.environ.get("HEADLINE_COPIES", "10"))
+N1, COPIES = 10_000_000, int(os.environ.get("HEADLINE_COPIES", "3"))
 exact = int(os.environ.get("HEADLINE_EXACT", "0"))
 ent = bench.load_system("zoom")
 S, N = ent["S"], N1*COPIES

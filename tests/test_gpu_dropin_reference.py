@@ -1,7 +1,7 @@
 """The drop-in wiring ON HARDWARE against the REAL reference.
 
-The reference (staged under oracle/_ref by oracle/make_ref.py, or
-/root/reference) runs on the host; its own ``GeometricTrace`` / ``System``
+The reference (staged under oracle/_ref by oracle/make_ref.py, or found
+through $RAYOPT_REFERENCE) runs on the host; its own ``GeometricTrace`` / ``System``
 classes are bound to the CUDA engine with ``rayopt_b200.bind`` /
 ``rayopt_b200.install`` and driven through the reference's own call patterns:
 
@@ -28,8 +28,8 @@ from conftest import assert_parity
 
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not ref_shim.available(),
-                                 reason="no reference tree (run oracle/make_ref.py where "
-                                        "/root/reference exists)")]
+                                 reason="no reference tree (oracle/make_ref.py stages one "
+                                        "from $RAYOPT_REFERENCE)")]
 
 
 @pytest.fixture(scope="module")

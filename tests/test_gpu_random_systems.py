@@ -147,8 +147,8 @@ def test_random_analytic_unrotated_bit_exact(eng, seed):
     # the default fast mode on ALL rays, no conditioning filter: it evaluates the
     # cancellation-prone analytic intercept with the reference's own roundings,
     # so even grazing / near-TIR / aperture-edge rays stay within 1e-10 with an
-    # identical NaN mask (measured worst 1.6e-12 over these seeds,
-    # profiles/r2e_fast_mode_conditioning.txt)
+    # identical NaN mask (tests/gpu_scripts/fast_mode_conditioning.py reports
+    # the worst error over these seeds)
     got = eng.trace(table, y0, u0, clip=clip)
     for a, b, w in zip(got, want, "yuit"):
         assert_parity(a, b, 1e-10, "seed %d fast %s" % (seed, w))

@@ -3,7 +3,7 @@
 // shared memory (the kernel's store path), read-only, and copy (the pattern
 // MEASURED_PEAKS.json's hbm_gbs was measured with).  CUDA events, 10 GB
 // buffers (>> 126 MB L2), best and median of 10.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o membw.bin membw.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o membw.bin membw.cu
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdio>

@@ -2,7 +2,7 @@
 // a tunable amount of dependent FP64 work, to separate memory-pattern effects
 // from compute effects.  Per warp tile (32*RPT rays): for s in 0..S-1:
 // D dependent DFMAs per ray, stage 10 values/ray, NARR bulk stores to row s.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tracelike.bin tracelike.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tracelike.bin tracelike.cu
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdio>
