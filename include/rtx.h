@@ -481,6 +481,60 @@ int rtx_focus_moments(rtx_ctx *ctx, int dtype, int64_t N, const void *y,
                       const void *inc, const void *w, const double *center,
                       double *m);
 
+/* ---- diffraction PSF (GeometricTrace.psf, rayopt/geometric_trace.py:133-169) */
+/*
+ * Linear interpolation of scattered values on a GIVEN triangulation -- the
+ * evaluation of griddata(method="linear", fill_value=nan)
+ * (geometric_trace.py:141) with the triangulation scipy.spatial.Delaunay made
+ * on the host.  All arrays are DEVICE arrays of `dtype` (RTX_F64 only; RTX_F32
+ * returns RTX_E_UNSUPPORTED):
+ *   pts (M,2) points, vals (M,) their values,
+ *   simplices (T,3) int32 and transform (T,3,2): Delaunay.simplices and
+ *     Delaunay.transform as they are (degenerate simplices keep their NaNs and
+ *     never cover a node),
+ *   gh (n,) the grid axis, 2 <= n <= 46340: node (i, j) is (gh[i], gh[j]),
+ *   out (n,n) receives the values, NaN where no simplex covers the node,
+ *   winner (n,n) int32 or NULL receives the covering simplex, the lowest
+ *     index among the simplices that cover the node within scipy's tolerance
+ *     (100 DBL_EPSILON in barycentric coordinates), INT32_MAX for none.
+ * The barycentric coordinates and the value follow scipy's evaluation order
+ * with unfused IEEE operations: a node whose covering simplex is the one
+ * Delaunay.find_simplex returns gets griddata's value bit for bit.
+ * Asynchronous; rtx_last_kernel_ms gives the device time of the call.
+ */
+int rtx_grid_linear(rtx_ctx *ctx, int dtype, int64_t M, const void *pts,
+                    const void *vals, int64_t T, const int32_t *simplices,
+                    const void *transform, int n, const void *gh, void *out,
+                    int32_t *winner);
+
+/*
+ * Device bytes an rtx_psf call on an (n,n) grid with zero padding `pad`
+ * allocates: the (pad n)^2 complex grid, plus cuFFT's work area unless the
+ * context's cached plan already has that shape.  RTX_E_UNSUPPORTED without
+ * cuFFT.
+ */
+int rtx_psf_bytes(rtx_ctx *ctx, int n, int pad, size_t *bytes);
+
+/*
+ * The diffraction PSF of a regridded OPD o (DEVICE (n,n), waves, NaN outside
+ * the pupil; RTX_F64 only):
+ *   z = where(isfinite(o), exp(-2 pi i o), 0)/sqrt(#finite), zero-padded at
+ *       the end to (nx, ny) = (pad n, pad n),
+ *   psf = |fft2(z)|^2/(nx ny)   DEVICE (nx, ny), unnormalised forward FFT.
+ * stats (host, 5 doubles, or NULL) receives #finite nodes, sum psf, max psf,
+ * and sum psf*k_p, sum psf*k_q with k the signed frequency index of
+ * np.fft.fftfreq along each axis (0, 1, .., -1): times 1/(nx d) these are the
+ * first moments about the frequency axes fftfreq(nx, d).  Sums are taken in a
+ * fixed order (the same inputs give the same bits).
+ * cuFFT (libcufft.so.11) is opened on the first call; without it the call
+ * returns RTX_E_UNSUPPORTED.  The plan of the last (nx, ny) and its work area
+ * are cached in the context.  When the complex grid and the work area do not
+ * fit in free device memory the call returns RTX_E_NOMEM before it allocates
+ * anything.  Synchronous.
+ */
+int rtx_psf(rtx_ctx *ctx, int dtype, int n, const void *o, int pad, void *psf,
+            double *stats);
+
 #ifdef __cplusplus
 }
 #endif

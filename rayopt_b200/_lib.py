@@ -69,6 +69,9 @@ SYMBOLS = {
     "rtx_ipc_close": (_i, [_vp, _vp]),
     "rtx_trace_gather": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _i64,
                               _u]),
+    "rtx_grid_linear": (_i, [_vp, _i, _i64, _vp, _vp, _i64, _vp, _vp, _i, _vp, _vp, _vp]),
+    "rtx_psf_bytes": (_i, [_vp, _i, _i, C.POINTER(_sz)]),
+    "rtx_psf": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
 }
 
 _lib = None
@@ -101,6 +104,40 @@ def load():
             lib.rtx_sizeof_aim(), aim_dtype().itemsize))
     _lib = lib
     return lib
+
+
+RTX_E_NOMEM = -3
+_cufft = None
+
+
+def preload_cufft():
+    """Load cuFFT (libcufft.so.11) with RTLD_GLOBAL so that librtx.so's own
+    dlopen by soname finds it: from the CUDA toolkit's lib64 ($CUDA_HOME,
+    $CUDA_PATH, /usr/local/cuda), else from the nvidia-cufft wheel that
+    torch installs.  librtx.so does not link against cuFFT; without it only
+    the PSF calls fail (RTX_E_UNSUPPORTED).  Returns the path loaded, or None."""
+    global _cufft
+    if _cufft is not None:
+        return _cufft
+    cands = [os.path.join(d, "lib64", "libcufft.so.11")
+             for d in (os.environ.get("CUDA_HOME"), os.environ.get("CUDA_PATH"), "/usr/local/cuda")
+             if d]
+    try:
+        import importlib.util
+        spec = importlib.util.find_spec("nvidia")
+        for d in (spec.submodule_search_locations or []) if spec else []:
+            cands.append(os.path.join(d, "cufft", "lib", "libcufft.so.11"))
+    except (ImportError, ValueError):
+        pass
+    for path in cands:
+        if os.path.exists(path):
+            try:
+                C.CDLL(path, mode=C.RTLD_GLOBAL)
+            except OSError:
+                continue
+            _cufft = path
+            return path
+    return None
 
 
 def check(code):

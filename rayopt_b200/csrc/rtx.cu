@@ -4,7 +4,10 @@
 //        -Xcompiler -fPIC -o librtx.so rtx.cu
 #include "../../include/rtx.h"
 #include "rtx_device.cuh"
+#include "rtx_psf.cuh"
 
+#include <cufft.h>  // types only: the library is opened at run time (rtx_psf)
+#include <dlfcn.h>
 #include <sched.h>
 #include <sys/syscall.h>
 #include <unistd.h>
@@ -93,6 +96,16 @@ struct rtx_ctx {
     cpu_set_t saved_affinity;
     bool tuned = false;       // an RTX_* environment knob overrides the heuristics
     int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
+    // rtx_grid_linear: claim grid when the caller wants no winner output
+    int* d_winner = nullptr;
+    size_t winner_cap = 0;
+    // rtx_psf: the cuFFT plan of the last (nx, ny) and its work area
+    cufftHandle fft_plan = 0;
+    bool fft_planned = false;
+    long long fft_nx = 0, fft_ny = 0;
+    void* fft_work = nullptr;
+    size_t fft_work_bytes = 0;
+    double* d_psf_red = nullptr;  // partial sums, the finite count and the stats
 };
 
 namespace {
@@ -610,6 +623,59 @@ void clear_chunk_events(rtx_ctx* ctx) {
     ctx->chunk_events.clear();
 }
 
+// cuFFT is opened at run time, so that librtx.so loads and traces on a machine
+// without it (the Python side preloads the toolkit's or the pip wheel's copy
+// with RTLD_GLOBAL; the soname lookup then finds that one)
+struct CufftApi {
+    bool ok = false;
+    cufftResult (*create)(cufftHandle*) = nullptr;
+    cufftResult (*set_auto_allocation)(cufftHandle, int) = nullptr;
+    cufftResult (*get_size_many64)(cufftHandle, int, long long*, long long*, long long, long long,
+                                   long long*, long long, long long, cufftType, long long,
+                                   size_t*) = nullptr;
+    cufftResult (*make_plan_many64)(cufftHandle, int, long long*, long long*, long long, long long,
+                                    long long*, long long, long long, cufftType, long long,
+                                    size_t*) = nullptr;
+    cufftResult (*set_work_area)(cufftHandle, void*) = nullptr;
+    cufftResult (*set_stream)(cufftHandle, cudaStream_t) = nullptr;
+    cufftResult (*exec_z2z)(cufftHandle, cufftDoubleComplex*, cufftDoubleComplex*, int) = nullptr;
+    cufftResult (*destroy)(cufftHandle) = nullptr;
+};
+
+const CufftApi& cufft_api() {
+    static const CufftApi api = [] {
+        CufftApi a;
+        void* h = dlopen("libcufft.so.11", RTLD_NOW | RTLD_GLOBAL);
+        if (!h) h = dlopen("libcufft.so", RTLD_NOW | RTLD_GLOBAL);
+        if (!h) return a;
+        bool all = true;
+        auto sym = [&](auto& fn, const char* name) {
+            fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(dlsym(h, name));
+            all = all && fn != nullptr;
+        };
+        sym(a.create, "cufftCreate");
+        sym(a.set_auto_allocation, "cufftSetAutoAllocation");
+        sym(a.get_size_many64, "cufftGetSizeMany64");
+        sym(a.make_plan_many64, "cufftMakePlanMany64");
+        sym(a.set_work_area, "cufftSetWorkArea");
+        sym(a.set_stream, "cufftSetStream");
+        sym(a.exec_z2z, "cufftExecZ2Z");
+        sym(a.destroy, "cufftDestroy");
+        a.ok = all;
+        return a;
+    }();
+    return api;
+}
+
+void release_fft_plan(rtx_ctx* ctx) {
+    if (ctx->fft_planned) cufft_api().destroy(ctx->fft_plan);
+    if (ctx->fft_work) cudaFree(ctx->fft_work);
+    ctx->fft_planned = false;
+    ctx->fft_work = nullptr;
+    ctx->fft_work_bytes = 0;
+    ctx->fft_nx = ctx->fft_ny = 0;
+}
+
 constexpr size_t SMALL_PATH_BYTES = 4u << 20;
 constexpr size_t ZERO_COPY_BYTES = 16u << 10;  // rays + results of a zero-copy small trace
 
@@ -772,7 +838,10 @@ const char* rtx_strerror(int code) {
     switch (code) {
         case RTX_OK: return "ok";
         case RTX_E_BADARG: return "rtx: bad argument";
-        case RTX_E_UNSUPPORTED: return "rtx: unsupported (too many aspheric coefficients / surfaces, or RTX_EXACT with FP32)";
+        case RTX_E_UNSUPPORTED:
+            return "rtx: unsupported (too many aspheric coefficients / surfaces, RTX_EXACT with FP32, "
+                   "FP32 in the PSF calls, or rtx_psf without a loadable cuFFT: libcufft.so.11 "
+                   "was not found by dlopen)";
         case RTX_E_NOMEM: return "rtx: out of memory";
         default: break;
     }
@@ -867,6 +936,9 @@ int rtx_free(rtx_ctx* ctx) {
     if (ctx->d_moments) cudaFree(ctx->d_moments);
     if (ctx->d_epi) cudaFree(ctx->d_epi);
     if (ctx->d_aim_offsets) cudaFree(ctx->d_aim_offsets);
+    if (ctx->d_winner) cudaFree(ctx->d_winner);
+    release_fft_plan(ctx);
+    if (ctx->d_psf_red) cudaFree(ctx->d_psf_red);
     if (ctx->small_host) cudaFreeHost(ctx->small_host);
     if (ctx->small_dev) cudaFree(ctx->small_dev);
     if (ctx->t0) cudaEventDestroy(ctx->t0);
@@ -1780,6 +1852,172 @@ int rtx_focus_moments(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const v
         CK(cudaGetLastError());
     }
     CK(cudaMemcpyAsync(m, ctx->d_moments, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- diffraction PSF (GeometricTrace.psf, rayopt/geometric_trace.py:133-169)
+extern "C" {
+
+int rtx_grid_linear(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, const void* vals,
+                    int64_t T, const int32_t* simplices, const void* transform, int n,
+                    const void* gh, void* out, int32_t* winner) {
+    // n <= 46340: node indices fit in int32
+    if (!ctx || M < 0 || T < 0 || T >= INT_MAX || n < 2 || n > 46340 || !gh || !out)
+        return RTX_E_BADARG;
+    if ((M > 0 && (!pts || !vals)) || (T > 0 && (!simplices || !transform))) return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    const long long nn = (long long)n * n;
+    int* claim = winner;
+    if (!claim) {
+        if ((size_t)nn * sizeof(int) > ctx->winner_cap) {
+            if (ctx->d_winner) CK(cudaFree(ctx->d_winner));
+            ctx->d_winner = nullptr;
+            ctx->winner_cap = 0;
+            CK(cudaMalloc((void**)&ctx->d_winner, (size_t)nn * sizeof(int)));
+            ctx->winner_cap = (size_t)nn * sizeof(int);
+        }
+        claim = ctx->d_winner;
+    }
+    long long grid = (nn + 255) / 256;
+    const long long cap = (long long)ctx->sm_count * 16;
+    if (grid > cap) grid = cap;
+    CK(cudaEventRecord(ctx->k0, ctx->stream));
+    fill_i32_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(claim, nn, INT_MAX);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    if (T > 0) {
+        grid_claim_kernel<<<(unsigned)((T + 255) / 256), 256, 0, ctx->stream>>>(
+            (const double*)pts, M, simplices, (const double*)transform, T, (const double*)gh, n,
+            claim);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
+    grid_eval_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(
+        (const double*)vals, simplices, (const double*)transform, (const double*)gh, n, claim,
+        (double*)out);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, ctx->stream));
+    ctx->kernel_timed = true;
+    return 0;
+}
+
+int rtx_psf_bytes(rtx_ctx* ctx, int n, int pad, size_t* bytes) {
+    if (!ctx || !bytes || n < 1 || pad < 1) return RTX_E_BADARG;
+    const long long nx = (long long)n * pad;
+    size_t b = (size_t)(nx * nx) * sizeof(double2);  // the complex grid
+    if (!(ctx->fft_planned && ctx->fft_nx == nx && ctx->fft_ny == nx)) {
+        const CufftApi& fft = cufft_api();
+        if (!fft.ok) return RTX_E_UNSUPPORTED;
+        cufftHandle h;
+        if (fft.create(&h) != CUFFT_SUCCESS) return RTX_E_UNSUPPORTED;
+        long long dims[2] = {nx, nx};
+        size_t ws = 0;
+        cufftResult r = fft.set_auto_allocation(h, 0);
+        if (r == CUFFT_SUCCESS)
+            r = fft.get_size_many64(h, 2, dims, nullptr, 1, 0, nullptr, 1, 0, CUFFT_Z2Z, 1, &ws);
+        fft.destroy(h);
+        if (r != CUFFT_SUCCESS) return r == CUFFT_ALLOC_FAILED ? RTX_E_NOMEM : RTX_E_UNSUPPORTED;
+        b += ws;
+    }
+    *bytes = b;
+    return 0;
+}
+
+int rtx_psf(rtx_ctx* ctx, int dtype, int n, const void* o, int pad, void* psf, double* stats) {
+    if (!ctx || n < 1 || pad < 1 || !o || !psf) return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64) return RTX_E_BADARG;
+    const CufftApi& fft = cufft_api();
+    if (!fft.ok) return RTX_E_UNSUPPORTED;
+    CK(cudaSetDevice(ctx->device));
+    const long long nx = (long long)n * pad, ny = nx, tot = nx * ny;
+    const size_t zbytes = (size_t)tot * sizeof(double2);
+    const bool cached = ctx->fft_planned && ctx->fft_nx == nx && ctx->fft_ny == ny;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    // what a new plan would give back
+    const size_t avail = free_b + (cached ? 0 : ctx->fft_work_bytes);
+    if (zbytes > avail) return RTX_E_NOMEM;  // nothing allocated, the cached plan kept
+    if (!cached) {
+        cufftHandle h;
+        if (fft.create(&h) != CUFFT_SUCCESS) return RTX_E_UNSUPPORTED;
+        long long dims[2] = {nx, ny};
+        size_t ws = 0;
+        cufftResult r = fft.set_auto_allocation(h, 0);
+        if (r == CUFFT_SUCCESS)
+            r = fft.get_size_many64(h, 2, dims, nullptr, 1, 0, nullptr, 1, 0, CUFFT_Z2Z, 1, &ws);
+        if (r == CUFFT_SUCCESS && zbytes + ws > avail) {
+            fft.destroy(h);
+            return RTX_E_NOMEM;
+        }
+        release_fft_plan(ctx);
+        if (r == CUFFT_SUCCESS)
+            r = fft.make_plan_many64(h, 2, dims, nullptr, 1, 0, nullptr, 1, 0, CUFFT_Z2Z, 1, &ws);
+        if (r != CUFFT_SUCCESS) {
+            fft.destroy(h);
+            return r == CUFFT_ALLOC_FAILED ? RTX_E_NOMEM : RTX_E_UNSUPPORTED;
+        }
+        if (ws && cudaMalloc(&ctx->fft_work, ws) != cudaSuccess) {
+            cudaGetLastError();
+            fft.destroy(h);
+            ctx->fft_work = nullptr;
+            return RTX_E_NOMEM;
+        }
+        if (fft.set_work_area(h, ctx->fft_work) != CUFFT_SUCCESS) {
+            fft.destroy(h);
+            release_fft_plan(ctx);
+            return RTX_E_UNSUPPORTED;
+        }
+        ctx->fft_plan = h;
+        ctx->fft_planned = true;
+        ctx->fft_nx = nx;
+        ctx->fft_ny = ny;
+        ctx->fft_work_bytes = ws;
+    }
+    if (fft.set_stream(ctx->fft_plan, ctx->stream) != CUFFT_SUCCESS) return RTX_E_UNSUPPORTED;
+    // partials (4 per block), the finite count, the 5 stats
+    const size_t red_doubles = 4 * PSF_RED_BLOCKS + 1 + 5;
+    if (!ctx->d_psf_red) CK(cudaMalloc((void**)&ctx->d_psf_red, red_doubles * sizeof(double)));
+    double* part = ctx->d_psf_red;
+    auto* count = reinterpret_cast<unsigned long long*>(part + 4 * PSF_RED_BLOCKS);
+    double* d_stats = part + 4 * PSF_RED_BLOCKS + 1;
+    struct Grid {  // the complex grid is freed on every return path
+        double2* z = nullptr;
+        ~Grid() { if (z) cudaFree(z); }
+    } g;
+    if (cudaMalloc((void**)&g.z, zbytes) != cudaSuccess) {
+        cudaGetLastError();
+        g.z = nullptr;
+        return RTX_E_NOMEM;
+    }
+    const long long nn = (long long)n * n;
+    auto blocks = [&](long long items, long long per_sm) {
+        long long b = (items + 255) / 256, cap = (long long)ctx->sm_count * per_sm;
+        return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
+    };
+    CK(cudaMemsetAsync(count, 0, sizeof(unsigned long long), ctx->stream));
+    CK(cudaEventRecord(ctx->k0, ctx->stream));
+    count_finite_kernel<<<blocks(nn, 8), 256, 0, ctx->stream>>>((const double*)o, nn, count);
+    pupil_kernel<<<blocks(tot, 16), 256, 0, ctx->stream>>>((const double*)o, n, nx, ny, count, g.z);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    if (fft.exec_z2z(ctx->fft_plan, (cufftDoubleComplex*)g.z, (cufftDoubleComplex*)g.z,
+                     CUFFT_FORWARD) != CUFFT_SUCCESS)
+        return RTX_E_UNSUPPORTED;
+    intensity_kernel<<<PSF_RED_BLOCKS, 256, 0, ctx->stream>>>(g.z, nx, ny, (double*)psf, part);
+    psf_stats_kernel<<<1, 1, 0, ctx->stream>>>(part, PSF_RED_BLOCKS, count, d_stats);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, ctx->stream));
+    ctx->kernel_timed = true;
+    if (stats)
+        CK(cudaMemcpyAsync(stats, d_stats, 5 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }

@@ -1,0 +1,236 @@
+// rtx_psf.cuh -- device side of the diffraction PSF (sm_90a, FP64):
+// GeometricTrace.psf (rayopt/geometric_trace.py:133-169) after the per-ray OPD.
+//
+//   regridding  griddata(method="linear") on a GIVEN Delaunay triangulation
+//               (simplices, transform of scipy.spatial.Delaunay), evaluated by
+//               rasterising the triangles: a claim pass (atomicMin of the
+//               simplex index per grid node) and an evaluation pass, so that
+//               the result does not depend on scheduling
+//   pupil       exp(-2 pi i o)/sqrt(#finite) into the zero-padded complex grid
+//   intensity   |fft|^2/(nx ny) and a deterministic reduction of sum, max and
+//               the first moments over the frequency indices
+//
+// The barycentric coordinates and the interpolated value use the evaluation
+// order of scipy's _qhull / interpnd (c_k accumulated from 0 in index order,
+// c_2 = (1 - c_0) - c_1, value = ((0 + c_0 v_0) + c_1 v_1) + c_2 v_2) with
+// unfused IEEE operations, so a node evaluated on the simplex scipy's
+// find_simplex returns is bit-identical to griddata.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <climits>
+#include <cfloat>
+
+namespace rtx {
+
+constexpr double GRID_EPS = 100.0 * DBL_EPSILON;  // scipy's inside tolerance
+constexpr int GRID_WARP_NODES = 64;   // a simplex whose box has more nodes is rasterised by a warp
+constexpr int PSF_RED_BLOCKS = 1024;  // fixed grid of the reduction: deterministic sums
+
+struct Bary {
+    double c0, c1, c2;
+};
+
+// scipy _barycentric_coordinates, ndim = 2; tr = {T00, T01, T10, T11, r0, r1}
+__device__ __forceinline__ Bary barycentric(const double* __restrict__ tr, double x, double y) {
+    const double dx = __dsub_rn(x, tr[4]), dy = __dsub_rn(y, tr[5]);
+    Bary b;
+    b.c0 = __dadd_rn(__dadd_rn(0.0, __dmul_rn(tr[0], dx)), __dmul_rn(tr[1], dy));
+    b.c1 = __dadd_rn(__dadd_rn(0.0, __dmul_rn(tr[2], dx)), __dmul_rn(tr[3], dy));
+    b.c2 = __dsub_rn(__dsub_rn(1.0, b.c0), b.c1);
+    return b;
+}
+
+__device__ __forceinline__ bool inside(double c) {  // NaN (degenerate simplex): outside
+    return c >= -GRID_EPS && c <= 1.0 + GRID_EPS;
+}
+
+__global__ void fill_i32_kernel(int* __restrict__ a, long long n, int v) {
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < n;
+         k += (long long)gridDim.x * blockDim.x)
+        a[k] = v;
+}
+
+// index range [lo, hi] of the grid nodes whose axis value may lie in
+// [vmin, vmax]: one node of margin on each side covers the rounding of the
+// division and scipy's eps, clamped to the grid
+__device__ __forceinline__ void node_range(double vmin, double vmax, double g0, double step, int n,
+                                           int& lo, int& hi) {
+    const double a = floor((vmin - g0) / step) - 1.0, b = ceil((vmax - g0) / step) + 1.0;
+    lo = a < 0.0 ? 0 : (a > n - 1 ? n : (int)a);
+    hi = b > n - 1 ? n - 1 : (b < 0.0 ? -1 : (int)b);
+}
+
+// claim pass: one lane per simplex; boxes of more than GRID_WARP_NODES nodes
+// (hull slivers) are rasterised by the whole warp, one such simplex at a time
+__global__ void __launch_bounds__(256) grid_claim_kernel(
+    const double* __restrict__ pts, long long M, const int* __restrict__ simp,
+    const double* __restrict__ transform, long long T, const double* __restrict__ gh, int n,
+    int* __restrict__ winner) {
+    const long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    const double g0 = gh[0], step = (gh[n - 1] - gh[0]) / (double)(n - 1);
+    int i0 = 0, i1 = -1, j0 = 0, j1 = -1;
+    const double* tr = transform + 6 * s;
+    if (s < T && tr[0] == tr[0]) {  // NaN transform: degenerate, never a winner (as in scipy)
+        const int a = simp[3 * s], b = simp[3 * s + 1], c = simp[3 * s + 2];
+        if (a >= 0 && a < M && b >= 0 && b < M && c >= 0 && c < M) {
+            const double xa = pts[2 * a], xb = pts[2 * b], xc = pts[2 * c];
+            const double ya = pts[2 * a + 1], yb = pts[2 * b + 1], yc = pts[2 * c + 1];
+            node_range(fmin(xa, fmin(xb, xc)), fmax(xa, fmax(xb, xc)), g0, step, n, i0, i1);
+            node_range(fmin(ya, fmin(yb, yc)), fmax(ya, fmax(yb, yc)), g0, step, n, j0, j1);
+        }
+    }
+    const int wi = i1 >= i0 ? i1 - i0 + 1 : 0, wj = j1 >= j0 ? j1 - j0 + 1 : 0;
+    const int cnt = wi * wj;  // n <= 46340: no int overflow
+    const bool big = cnt > GRID_WARP_NODES;
+    if (!big) {
+        for (int i = i0; i <= i1; ++i)
+            for (int j = j0; j <= j1; ++j) {
+                const Bary c = barycentric(tr, gh[i], gh[j]);
+                if (inside(c.c0) && inside(c.c1) && inside(c.c2))
+                    atomicMin(winner + (long long)i * n + j, (int)s);
+            }
+    }
+    unsigned todo = __ballot_sync(0xffffffffu, big);
+    while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const long long ss = __shfl_sync(0xffffffffu, s, src);
+        const int bi = __shfl_sync(0xffffffffu, i0, src), bj = __shfl_sync(0xffffffffu, j0, src);
+        const int bwj = __shfl_sync(0xffffffffu, wj, src);
+        const int bcnt = __shfl_sync(0xffffffffu, cnt, src);
+        const double* btr = transform + 6 * ss;
+        for (int k = lane; k < bcnt; k += 32) {
+            const int i = bi + k / bwj, j = bj + k % bwj;
+            const Bary c = barycentric(btr, gh[i], gh[j]);
+            if (inside(c.c0) && inside(c.c1) && inside(c.c2))
+                atomicMin(winner + (long long)i * n + j, (int)ss);
+        }
+    }
+}
+
+// evaluation pass: the winning simplex's barycentric interpolation, NaN
+// (griddata's fill_value) where no simplex claimed the node
+__global__ void __launch_bounds__(256) grid_eval_kernel(
+    const double* __restrict__ vals, const int* __restrict__ simp,
+    const double* __restrict__ transform, const double* __restrict__ gh, int n,
+    const int* __restrict__ winner, double* __restrict__ out) {
+    const long long nn = (long long)n * n;
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < nn;
+         k += (long long)gridDim.x * blockDim.x) {
+        const int w = winner[k];
+        double v = CUDART_NAN;
+        if (w != INT_MAX) {
+            const Bary c = barycentric(transform + 6 * (long long)w, gh[k / n], gh[k % n]);
+            const int* sv = simp + 3 * (long long)w;
+            v = __dadd_rn(0.0, __dmul_rn(c.c0, vals[sv[0]]));
+            v = __dadd_rn(v, __dmul_rn(c.c1, vals[sv[1]]));
+            v = __dadd_rn(v, __dmul_rn(c.c2, vals[sv[2]]));
+        }
+        out[k] = v;
+    }
+}
+
+// number of finite nodes of the regridded OPD (integer atomics: deterministic)
+__global__ void __launch_bounds__(256) count_finite_kernel(const double* __restrict__ o, long long nn,
+                                                           unsigned long long* __restrict__ count) {
+    unsigned long long c = 0;
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < nn;
+         k += (long long)gridDim.x * blockDim.x)
+        c += isfinite(o[k]) ? 1ull : 0ull;
+    for (int off = 16; off; off >>= 1) c += __shfl_down_sync(0xffffffffu, c, off);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
+}
+
+// the zero-padded pupil function: np.where(good, exp(-2j pi o), 0)/sqrt(count)
+// in the top-left n x n corner of the (nx, ny) array (fft2(o, (nx, ny)) pads
+// at the end); numpy's complex division by the real sqrt(count) multiplies by
+// its reciprocal
+__global__ void __launch_bounds__(256) pupil_kernel(const double* __restrict__ o, int n, long long nx,
+                                                    long long ny,
+                                                    const unsigned long long* __restrict__ count,
+                                                    double2* __restrict__ out) {
+    const double scl = __ddiv_rn(1.0, __dsqrt_rn((double)*count));
+    const long long tot = nx * ny;
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < tot;
+         k += (long long)gridDim.x * blockDim.x) {
+        const long long I = k / ny, J = k % ny;
+        double2 z = make_double2(0.0, 0.0);
+        if (I < n && J < n) {
+            const double v = o[I * n + J];
+            double re = 0.0, im = 0.0;
+            if (isfinite(v)) sincos(__dmul_rn(-6.283185307179586, v), &im, &re);
+            z = make_double2(__dmul_rn(re, scl), __dmul_rn(im, scl));
+        }
+        out[k] = z;
+    }
+}
+
+// signed frequency index of np.fft.fftfreq(m): 0 .. (m-1)/2, then -(m/2) .. -1
+__device__ __forceinline__ double freq_index(long long i, long long m) {
+    return (double)(i < (m - 1) / 2 + 1 ? i : i - m);
+}
+
+// psf = |z|^2/(nx ny) and per-block partials {sum, max, sum psf k_p, sum psf k_q}
+// in a fixed order (grid of PSF_RED_BLOCKS blocks)
+__global__ void __launch_bounds__(256) intensity_kernel(const double2* __restrict__ z, long long nx,
+                                                        long long ny, double* __restrict__ psf,
+                                                        double* __restrict__ part) {
+    const long long tot = nx * ny;
+    const double size = (double)tot;
+    double s = 0.0, mx = -CUDART_INF, sp = 0.0, sq = 0.0;
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < tot;
+         k += (long long)gridDim.x * blockDim.x) {
+        const double2 a = z[k];
+        const double v = __ddiv_rn(__dadd_rn(__dmul_rn(a.x, a.x), __dmul_rn(a.y, a.y)), size);
+        psf[k] = v;
+        s += v;
+        mx = fmax(mx, v);
+        sp += v * freq_index(k / ny, nx);
+        sq += v * freq_index(k % ny, ny);
+    }
+    for (int off = 16; off; off >>= 1) {
+        s += __shfl_down_sync(0xffffffffu, s, off);
+        mx = fmax(mx, __shfl_down_sync(0xffffffffu, mx, off));
+        sp += __shfl_down_sync(0xffffffffu, sp, off);
+        sq += __shfl_down_sync(0xffffffffu, sq, off);
+    }
+    __shared__ double sh[4][8];
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) {
+        sh[0][w] = s;
+        sh[1][w] = mx;
+        sh[2][w] = sp;
+        sh[3][w] = sq;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double r[4] = {0.0, -CUDART_INF, 0.0, 0.0};
+        for (int k = 0; k < (int)(blockDim.x >> 5); ++k) {
+            r[0] += sh[0][k];
+            r[1] = fmax(r[1], sh[1][k]);
+            r[2] += sh[2][k];
+            r[3] += sh[3][k];
+        }
+        for (int q = 0; q < 4; ++q) part[4 * blockIdx.x + q] = r[q];
+    }
+}
+
+// stats = {#finite, sum, max, sum psf k_p, sum psf k_q} from the partials, one
+// thread in block order
+__global__ void psf_stats_kernel(const double* __restrict__ part, int nblocks,
+                                 const unsigned long long* __restrict__ count,
+                                 double* __restrict__ stats) {
+    double r[4] = {0.0, -CUDART_INF, 0.0, 0.0};
+    for (int b = 0; b < nblocks; ++b) {
+        r[0] += part[4 * b];
+        r[1] = fmax(r[1], part[4 * b + 1]);
+        r[2] += part[4 * b + 2];
+        r[3] += part[4 * b + 3];
+    }
+    stats[0] = (double)*count;
+    for (int q = 0; q < 4; ++q) stats[1 + q] = r[q];
+}
+
+}  // namespace rtx

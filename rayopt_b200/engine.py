@@ -611,6 +611,88 @@ class Engine:
         m = mom(m[2:6]/m[0])
         return float(-m[6]/m[7])
 
+    # ---- diffraction PSF (GeometricTrace.psf, rayopt/geometric_trace.py:133-169)
+    def grid_linear(self, points, values, tri, n, gh, download=True, winner=False):
+        """rtx_grid_linear: griddata(points, values, (xs, ys), method="linear",
+        fill_value=nan) on the grid node (i, j) = (gh[i], gh[j]), with the
+        host triangulation `tri` (scipy.spatial.Delaunay of `points`).
+        Returns the (n, n) values -- numpy, or a DeviceArray when not
+        `download` -- and with `winner` also the covering simplex per node
+        (numpy int32, -1 where none covers it, like find_simplex)."""
+        points = np.ascontiguousarray(points, np.float64)
+        values = np.ascontiguousarray(values, np.float64)
+        gh = np.ascontiguousarray(gh, np.float64)
+        if points.ndim != 2 or points.shape[1] != 2 or values.shape != points.shape[:1]:
+            raise ValueError("points must be (M, 2) and values (M,)")
+        if gh.shape != (int(n),):
+            raise ValueError("gh must be the (n,) grid axis")
+        n = int(n)
+        simp = np.ascontiguousarray(tri.simplices, np.int32)
+        tr = np.ascontiguousarray(tri.transform, np.float64)
+        ins = [self.to_device(a) for a in (points, values, simp, tr, gh)]
+        out = self.empty((n, n))
+        win = self.empty((n, n), np.int32) if winner else None
+        try:
+            check(self.lib.rtx_grid_linear(self.ctx, RTX_F64, len(points), ins[0].ptr, ins[1].ptr,
+                                           len(simp), ins[2].ptr, ins[3].ptr, n, ins[4].ptr,
+                                           out.ptr, None if win is None else win.ptr))
+            w = None
+            if win is not None:
+                w = win.download()
+                w[w == np.iinfo(np.int32).max] = -1
+                win.free()
+            if download:
+                o = out.download()
+                out.free()
+                out = o
+            else:
+                self.sync()
+        finally:
+            for a in ins:
+                a.free()
+        return (out, w) if winner else out
+
+    def psf_bytes(self, n, pad):
+        """device bytes rtx_psf allocates for itself on an (n, n) grid"""
+        _lib.preload_cufft()
+        b = C.c_size_t()
+        check(self.lib.rtx_psf_bytes(self.ctx, int(n), int(pad), C.byref(b)))
+        return b.value
+
+    def psf(self, o, pad):
+        """rtx_psf of the regridded OPD `o` (DEVICE (n, n) FP64): the
+        (pad n, pad n) PSF |fft2(exp(-2 pi i o)/sqrt(#finite))|^2/(pad n)^2 as
+        a DeviceArray, and the device's raw stats (#finite, sum, max,
+        sum psf k_p, sum psf k_q; include/rtx.h) for ``psf_stats``.  Raises
+        RtxError (RTX_E_NOMEM) before allocating anything when the PSF and
+        the library's buffers do not fit in free device memory."""
+        n, pad = int(o.shape[0]), int(pad)
+        if o.shape != (n, n) or o.dtype != np.float64:
+            raise ValueError("o must be a square FP64 device array")
+        nx = n*pad
+        free = self.free_bytes()
+        # the complex grid and the PSF alone, then with cuFFT's work area
+        if nx*nx*(16 + 8) > free or self.psf_bytes(n, pad) + nx*nx*8 > free:
+            check(_lib.RTX_E_NOMEM)
+        out = self.empty((nx, nx))
+        raw = np.zeros(5)
+        try:
+            check(self.lib.rtx_psf(self.ctx, RTX_F64, n, o.ptr, pad, out.ptr, ptr(raw)))
+        except Exception:
+            out.free()
+            raise
+        return out, raw
+
+    @staticmethod
+    def psf_stats(raw, f):
+        """count, sum, peak and the first moments sum psf*p, sum psf*q of a
+        PSF on the frequency axis `f` (np.fft.fftfreq(nx, d)) from the raw
+        device stats of ``psf``"""
+        nx = len(f)
+        step = f[1] if nx > 1 else 0.        # fftfreq: f[k] = k/(nx d)
+        return dict(count=int(raw[0]), sum=float(raw[1]), max=float(raw[2]),
+                    cp=float(raw[3]*step), cq=float(raw[4]*step))
+
 
 _default = {}
 

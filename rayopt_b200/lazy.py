@@ -414,6 +414,67 @@ class ResidentMixin:
             x, y = xs, ys
         return x, y, t
 
+    # ---- diffraction PSF with the regridding and the FFT on the device
+    def _opd_grid(self, radius, after, image, resample, download):
+        """opd's regridding on the device: the host triangulates the finite
+        exit-pupil points (scipy.spatial.Delaunay, griddata's own options),
+        rtx_grid_linear interpolates on the reference's grid"""
+        from scipy.spatial import Delaunay
+        x, y, t = self.opd_rays(radius, after, image)
+        ok = np.isfinite(x) & np.isfinite(y) & np.isfinite(t)
+        x, y, t = x[ok], y[ok], t[ok]
+        if not t.size:
+            raise ValueError("no rays made it through")
+        n = int(resample*self.nrays**.5)
+        h = np.fabs((x, y)).max()
+        xs, ys = np.mgrid[-1:1:1j*n, -1:1:1j*n]*h
+        pts = np.stack([x, y], axis=-1)
+        o = self._engine().grid_linear(pts, t, Delaunay(pts), n, xs[:, 0].copy(),
+                                       download=download)
+        return xs, ys, o
+
+    def opd_device(self, radius=None, after=-2, image=-1, resample=4):
+        """``opd`` (rayopt/geometric_trace.py:101-144) with the regridding on
+        the device (rtx_grid_linear on the host's Delaunay triangulation):
+        griddata's values bit for bit wherever the device picks the simplex
+        scipy's find_simplex picks; nodes on shared edges may take the
+        neighbour's value (equal to rounding)"""
+        if not resample:
+            return self.opd_rays(radius, after, image)
+        return self._opd_grid(radius, after, image, resample, download=True)
+
+    def psf_device(self, pad=4, resample=4, download=True, **kwargs):
+        """``psf`` (rayopt/geometric_trace.py:146-169) on the device: the
+        regridded OPD stays in HBM, the pupil function, the padded FFT
+        (cuFFT) and |.|^2 run there (rtx_psf).  Returns (p, q, psf) like the
+        reference; with ``download=False`` psf is a DeviceArray (free it when
+        done) and ``self.psf_stats`` holds its count of finite pupil nodes,
+        sum, peak and centroid sums (cp, cq) = (sum psf*p, sum psf*q) from a
+        device reduction"""
+        if not resample:
+            raise NotImplementedError       # as in the reference
+        eng = self._engine()
+        radius = self.system[-1].distance
+        after, image = kwargs.pop("after", -2), kwargs.pop("image", -1)
+        if kwargs:
+            raise TypeError("unexpected arguments %s" % sorted(kwargs))
+        xs, ys, o = self._opd_grid(radius, after, image, resample, download=False)
+        try:
+            out, raw = eng.psf(o, pad)
+        finally:
+            o.free()
+        nx = pad*xs.shape[0]
+        dx = xs[1, 0] - xs[0, 0]
+        k = 1/(self.l/self.system.scale)
+        f = np.fft.fftfreq(nx, dx*k/radius)
+        p, q = np.broadcast_arrays(f[:, None], f)
+        self.psf_stats = eng.psf_stats(raw, f)
+        if download:
+            psf = out.download()
+            out.free()
+            return p, q, psf
+        return p, q, out
+
 
 class ResidentTrace(ResidentMixin):
     """Standalone resident drop-in (no rayopt import needed) with launch rays
