@@ -541,6 +541,25 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
         }
     }
     if (!(aligned && fits(rpt))) store = STORE_DIRECT;  // per-ray stores: exactly N rays
+    // a long table leaves less shared memory for the staging buffers (256 FP64
+    // surfaces take 92 KB): step down to the smallest staged kernel, then to
+    // per-ray stores, rather than refuse a table the library accepts
+    auto smem_of = [&](int r, int st, int w, int nb) {
+        return r == 4 ? trace_smem_bytes<T, 4>(S, st, w, nb)
+                      : r == 2 ? trace_smem_bytes<T, 2>(S, st, w, nb)
+                               : trace_smem_bytes<T, 1>(S, st, w, nb);
+    };
+    const size_t optin = (size_t)ctx->max_smem_optin;
+    if (!ctx->tuned && store != STORE_DIRECT && smem_of(rpt, store, warps, nbuf) > optin) {
+        if (fits(1) && smem_of(1, STORE_WARP, 8, 2) <= optin) {
+            rpt = 1;
+            store = STORE_WARP;
+            warps = 8;
+            nbuf = 2;
+        } else {
+            store = STORE_DIRECT;
+        }
+    }
     if (batch && batch->n > 0) {
         p.nbatch = batch->n;
         for (int b = 0; b < batch->n; ++b) p.item[b] = batch->item[b];

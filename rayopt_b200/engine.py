@@ -29,6 +29,24 @@ def _code(dtype):
         raise TypeError("dtype must be float64 or float32, got %r" % (dtype,))
 
 
+def _check_operands(dtype, N, **arrays):
+    """The reductions and epilogues take their element type from the rays and
+    read N rays from every other array: each (DeviceArray, values per ray)
+    in `arrays` (None entries are skipped) must have that dtype and room for N
+    rays.  Raises ValueError before anything is launched."""
+    dtype = np.dtype(dtype)
+    if N < 0:
+        raise ValueError("N must be >= 0, got %d" % N)
+    for name, (a, per_ray) in arrays.items():
+        if a is None:
+            continue
+        if np.dtype(a.dtype) != dtype:
+            raise ValueError("%s is %s but the rays are %s" % (name, np.dtype(a.dtype), dtype))
+        room = a.nbytes//(dtype.itemsize*per_ray)
+        if N > room:
+            raise ValueError("N = %d rays but %s holds only %d" % (N, name, room))
+
+
 class DeviceArray:
     """A typed block of HBM owned by an Engine (freed with it or on .free())."""
 
@@ -382,6 +400,7 @@ class Engine:
         (y_x, y_y, u_x, u_y) guess centres (e.g. the chief ray's)."""
         table = self._table(table)
         N = y0.shape[0] if N is None else int(N)
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3), w=(w, 1))
         r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         c = None if center is None else np.ascontiguousarray(center, np.float64).reshape(4)
         m = np.zeros(20)
@@ -430,6 +449,7 @@ class Engine:
         (include/rtx.h); A (N,), P (N,3) DeviceArrays.  Asynchronous."""
         table = self._table(table)
         N = y0.shape[0] if N is None else int(N)
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3), A=(A, 1), P=(P, 3))
         r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         rec = np.zeros(1, OPD_DTYPE)
         for k in ("y0_ref", "u0_ref", "M", "d"):
@@ -566,6 +586,7 @@ class Engine:
         (include/rtx.h rtx_moments): 8 doubles."""
         m = np.zeros(8)
         N = y.shape[-2] if N is None else int(N)
+        _check_operands(y.dtype, N, y=(y, 3), w=(w, 1))
         c = None if center is None else np.ascontiguousarray(center, np.float64)
         check(self.lib.rtx_moments(self.ctx, _code(y.dtype), N, y.ptr,
                                    None if w is None else w.ptr, ptr(c), ptr(m)))
@@ -598,6 +619,7 @@ class Engine:
         `comm_sum` all-reduces the 8 moments for ray-sharded bundles."""
         red = comm_sum or (lambda v: v)
         N = y.shape[-2] if N is None else int(N)
+        _check_operands(y.dtype, N, y=(y, 3), inc=(inc, 3), w=(w, 1))
 
         def mom(center):
             m = np.zeros(8)
