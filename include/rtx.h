@@ -70,7 +70,14 @@ extern "C" {
 #define RTX_STORE_DIRECT 2u /* debug: force per-thread strided stores instead
                                of the shared-memory staged bulk (TMA) stores */
 #define RTX_RPT1       4u /* tuning: one ray per thread  (default: library's choice) */
-#define RTX_RPT2       8u /* tuning: two rays per thread */
+#define RTX_RPT2       8u /* tuning: two rays per thread.  An explicit RPT is
+                             honoured at every N wherever the pitch and the
+                             output alignment allow it (ld a multiple of 32*RPT,
+                             16-byte aligned outputs, a table that leaves room
+                             for the staging buffers); elsewhere the launch
+                             steps down as it does for its own choice.  The
+                             results never depend on the kernel chosen
+                             (rtx_last_launch_config reports it). */
 #define RTX_GATHER_XY 16u /* rtx_trace_gather: the intercept buffers dst[k] are
                              (Ntotal, 2) arrays receiving x,y only -- what a spot
                              diagram reads (rayopt/analysis.py:274): 16 instead of
@@ -174,6 +181,12 @@ int64_t rtx_launch_count(rtx_ctx *ctx);
 /* CTAs the most recent trace kernel launch ran with (a persistent grid: one
  * resident wave, fewer when clusters of CTAs leave SMs unused) */
 int rtx_last_launch_ctas(rtx_ctx *ctx, int *ctas);
+/* configuration of the most recent trace kernel launch: cfg = {rays per
+ * thread, store path (0 per-thread, 1 per-warp bulk, 2 per-CTA bulk), warps
+ * per CTA, staging buffers, CTAs per cluster as launched (1 where the
+ * clustered kernel fell back to the per-CTA one)}.  All zero before the first
+ * launch. */
+int rtx_last_launch_config(rtx_ctx *ctx, int cfg[5]);
 
 /* ---- the hot path ------------------------------------------------------ */
 /*

@@ -45,6 +45,7 @@ SYMBOLS = {
     "rtx_last_kernel_ms": (_i, [_vp, C.POINTER(C.c_float)]),
     "rtx_launch_count": (_i64, [_vp]),
     "rtx_last_launch_ctas": (_i, [_vp, C.POINTER(_i)]),
+    "rtx_last_launch_config": (_i, [_vp, C.POINTER(_i)]),
     "rtx_trace": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _i, _i64,
                        _vp, _vp, _vp, _vp, _u]),
     "rtx_trace_batch": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i64,

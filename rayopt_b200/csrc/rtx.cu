@@ -88,6 +88,7 @@ struct rtx_ctx {
     int cluster = 1;          // CTAs per cluster of the per-CTA store kernel (RTX_CLUSTER)
     int max_ctas_per_sm = 0;  // 0: whatever fits
     int last_ctas = 0;        // CTAs of the last trace launch (rtx_last_launch_ctas)
+    int last_cfg[5] = {0, 0, 0, 0, 0};  // rpt, store, warps, nbuf, cluster (rtx_last_launch_config)
     unsigned* mask = nullptr; // rtx_set_mask_output
     void* tsum = nullptr;     // rtx_set_path_sum_output
     int tsum_upto = 0;
@@ -238,6 +239,8 @@ int launch_one(rtx_ctx* ctx, const TraceParams<T>& p, cudaStream_t stream) {
         ctx->last_ctas = (int)grid;
         kern<<<(unsigned)grid, threads, smem, stream>>>(q);
     }
+    const int cfg[5] = {RPT, STORE, WARPS, NBUF, CLUSTER};
+    memcpy(ctx->last_cfg, cfg, sizeof(cfg));
     ctx->launches++;
     return (int)cudaGetLastError();
 }
@@ -482,7 +485,9 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
             warps = 16;
         }
     }
-    if (N <= 150 * 1000 && !ctx->tuned) {
+    // (an explicit RPT request is honoured at every N; the pitch and alignment
+    // step-downs below still apply to it)
+    if (N <= 150 * 1000 && !ctx->tuned && !explicit_rpt) {
         // small bundles: 256-ray warp tiles spread over all SMs
         rpt = 1;
         store = STORE_WARP;
@@ -502,7 +507,7 @@ int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot
         store = STORE_CTA;
         warps = 8;
         nbuf = 1;
-    } else if (N <= 32 * 1024) {  // (tuned contexts keep the old small-bundle rule)
+    } else if (N <= 32 * 1024 && !explicit_rpt) {  // (tuned contexts keep the old small-bundle rule)
         rpt = 1;
         store = STORE_WARP;
         warps = 8;
@@ -1133,6 +1138,11 @@ int64_t rtx_launch_count(rtx_ctx* ctx) { return ctx ? ctx->launches : 0; }
 int rtx_last_launch_ctas(rtx_ctx* ctx, int* ctas) {
     if (!ctx || !ctas) return RTX_E_BADARG;
     *ctas = ctx->last_ctas;
+    return 0;
+}
+int rtx_last_launch_config(rtx_ctx* ctx, int cfg[5]) {
+    if (!ctx || !cfg) return RTX_E_BADARG;
+    memcpy(cfg, ctx->last_cfg, sizeof(ctx->last_cfg));
     return 0;
 }
 

@@ -231,6 +231,15 @@ class Engine:
         check(self.lib.rtx_last_launch_ctas(self.ctx, C.byref(n)))
         return n.value
 
+    def last_launch_config(self):
+        """(rpt, store, warps, nbuf, cluster) of the most recent trace kernel
+        launch: rays per thread, store path (0 per-thread, 1 per-warp bulk,
+        2 per-CTA bulk), warps per CTA, staging buffers, CTAs per cluster as
+        launched"""
+        cfg = (C.c_int*5)()
+        check(self.lib.rtx_last_launch_config(self.ctx, cfg))
+        return tuple(cfg)
+
     # ---- the hot path -------------------------------------------------
     @staticmethod
     def _table(table):

@@ -17,21 +17,14 @@ launch rays with rtx_trace and checks the epilogues against the stored rows:
 
 The reduce sums through atomicAdd, so it is not asserted to repeat bit for bit.
 
-One configuration does not share the stored state bit for bit: Newton
-(aspheric) systems in fast FP64 and FP32 mode, where rtx_trace runs its
-one-ray-per-thread kernel -- by default for bundles up to 150 000 rays, and
-wherever RTX_RPT or an explicit RPT selects it.  Measured on an H100
-(cooke_asph, keep-LAST): the epilogue (two rays per thread) agrees bit for bit
-with rtx_trace's two- and four-ray kernels at every size, and RTX_EXACT agrees
-in every configuration; against the one-ray kernel a few rays in a thousand
-differ by a few ulps (|dA| <= 9e-14 in FP64, <= 5e-5 in FP32 for |A| ~ 100 mm;
-FP32 moments up to ~70 ulps of sum|term|, FP32 Newton stopping within 4 ulps
-of the step).  Spelling out the Newton step's FMAs and rounded products did
-not remove the difference, so its cause lies elsewhere in the one-ray
-instantiation and is not established here.  Newton systems in fast and FP32
-mode therefore allow 64 ulps of FP64, 256 of FP32, per term instead of bit
-identity, at every N so that the allowance does not depend on which kernel
-the library picks.
+This holds for Newton (aspheric) systems in fast FP64 and FP32 mode too, with
+no per-ray allowance.  The one-ray-per-thread trace kernel used to differ
+there from the two- and four-ray kernels and from the epilogue by a few ulps
+for a few rays in a thousand: the Newton slope's r2 = x*x + y*y (and the
+normal's q_x^2 + q_y^2 + 1) were plain expressions, and the compiler fused a
+different one of the two products in that kernel.  Both are now written with
+one explicit rounded product and one FMA (rtx_device.cuh, sumsq2_fast);
+tests/test_gpu_config_invariance.py pins every configuration to the same bits.
 """
 import ctypes as C
 
@@ -122,14 +115,13 @@ def _L_mom(eng, N):
     return -(-N//(256*blocks)) + blocks
 
 
-def _within(got, want, scale, L, what, state_eps=0.):
-    """|got - want| <= ((L + 64) eps + 64 state_eps) scale elementwise (NaN
-    where want is NaN); state_eps: the per-ray state's own difference, see the
-    module docstring.  Returns the worst ratio to the bound"""
+def _within(got, want, scale, L, what):
+    """|got - want| <= (L + 64) eps scale elementwise (NaN where want is NaN).
+    Returns the worst ratio to the bound"""
     got, want, scale = (np.asarray(a, np.float64) for a in (got, want, scale))
     nan = np.isnan(want)
     assert np.array_equal(np.isnan(got), nan), (what, got, want)
-    tol = ((L + 64)*EPS + 64*state_eps)*scale[~nan]
+    tol = (L + 64)*EPS*scale[~nan]
     err = np.abs(got[~nan] - want[~nan])
     assert np.all(err <= tol), (what, np.flatnonzero(~nan)[err > tol], got, want)
     return float(np.max(err/np.where(tol > 0, tol, 1), initial=0.))
@@ -194,28 +186,17 @@ def _stored(eng, table, dy0, du0, N, dtype, exact, clip, rot0, rows="last", path
     return out + [p]
 
 
-def _state_eps(table, dtype, exact):
-    """0 where the epilogue sees rtx_trace's state bit for bit, else the
-    allowance of the module docstring (Newton systems, fast or FP32): 1 ulp of
-    FP64, 4 of FP32 (FP32 Newton stops within 4 ulps of the step)"""
-    if exact or not (table["n_asph"] >= 0).any():
-        return 0.
-    return float(np.finfo(dtype).eps)*(4 if dtype == np.float32 else 1)
-
-
 def _check_reduce(eng, table, dy0, du0, N, dtype, exact, clip, rot0, w, center, y, inc):
     """rtx_trace_reduce and rtx_moments / rtx_focus_moments on the stored rows
     against the exact sums of the stored rows; returns the worst ratio"""
-    se = _state_eps(table, dtype, exact)
     m = eng.trace_reduce(table, dy0, du0, N=N, clip=clip, rot0=rot0, exact=exact,
                          w=w, center=center)
     wh = None if w is None else w.download()[:N]
     s, a = epi_oracle.reduce_sums(y, inc, wh, center)
     for k in (4, 5, 8):
         assert m[k] == s[k], (k, m[k], s[k])
-    worst = _within(m, s, a, _L_epi(eng, N), "trace_reduce", se)
-    _derived(m, s, a, w is None, center, max(1e-12, 1e3*se), max(1e-10, 1e3*se),
-             "vs stored rows")
+    worst = _within(m, s, a, _L_epi(eng, N), "trace_reduce")
+    _derived(m, s, a, w is None, center, 1e-12, 1e-10, "vs stored rows")
     # the same sums from the stored rows by the two stand-alone kernels
     if N:
         dy, di = eng.to_device(y, dtype), eng.to_device(inc, dtype)
@@ -270,16 +251,9 @@ def _check_opd(eng, table, dy0, du0, y0, u0, N, dtype, exact, clip, rot0, k):
         return
     wa, wp = epi_oracle.opd_epilogue(y0[:N].astype(dtype), Y[0], U[0], ps, spec)
     assert a.dtype == wa.dtype
-    se = _state_eps(table, dtype, exact)
-    if se:
-        for g, w_ in ((a[:N], wa), (p[:N], wp)):
-            assert np.array_equal(np.isnan(g), np.isnan(w_))
-            ok = ~np.isnan(w_)
-            assert np.all(np.abs(g[ok] - w_[ok]) <= 64*se*np.abs(w_[ok]).max(initial=0.))
-    else:
-        assert np.array_equal(a[:N], wa, equal_nan=True), np.flatnonzero(
-            ~((a[:N] == wa) | (np.isnan(a[:N]) & np.isnan(wa))))[:8]
-        assert np.array_equal(p[:N], wp, equal_nan=True)
+    assert np.array_equal(a[:N], wa, equal_nan=True), np.flatnonzero(
+        ~((a[:N] == wa) | (np.isnan(a[:N]) & np.isnan(wa))))[:8]
+    assert np.array_equal(p[:N], wp, equal_nan=True)
     if dtype == np.float64 and N <= 70001:
         T = eng.trace(table, y0[:N], u0[:N], clip=clip, rot0=rot0, exact=exact, want=("t",))[3]
         T = np.vstack([np.zeros((1, N)), T])            # row 0: the launch, t = 0
