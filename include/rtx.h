@@ -207,8 +207,10 @@ int rtx_last_launch_config(rtx_ctx *ctx, int cfg[5]);
  *           arrays Y,U,I: (rows, ld, 3), T: (rows, ld); rows = S or 1.
  *           With ld a multiple of 128 rays (64 suffices in FP64) the kernel
  *           uses staged bulk (TMA) stores and writes whole groups of 32 x
- *           rays-per-thread rays (columns N..ld-1 are padding and receive
- *           unspecified values); a multiple of 32 or 64 selects a kernel with
+ *           rays-per-thread rays: columns N .. up(N, 32 rpt)-1 are padding
+ *           and receive unspecified values, and nothing at or after column
+ *           up(N, 32 rpt) of a row is written (rpt as rtx_last_launch_config
+ *           reports it); a multiple of 32 or 64 selects a kernel with
  *           fewer rays per thread; any other ld takes the per-thread store
  *           path and touches only columns < N.
  *           Y: intercepts, U: excidence, I: incidence directions (unclipped),
@@ -270,6 +272,10 @@ int rtx_set_mask_output(rtx_ctx *ctx, uint32_t *dmask);
  * receives sum over traced surfaces 0..upto (inclusive; upto < 0: all) of
  * t -- the accumulation GeometricTrace.opd starts from
  * (rayopt/geometric_trace.py:102), without reading the (S,N) array again.
+ * The sum is taken left to right over the t values as they are stored (each
+ * rounded to the trace dtype), so it is bit-identical to adding the stored
+ * T rows 0..upto in order, in every mode and kernel configuration.  Only
+ * entries 0..N-1 are written.
  */
 int rtx_set_path_sum_output(rtx_ctx *ctx, void *dsum, int upto);
 

@@ -47,6 +47,31 @@ def _check_operands(dtype, N, **arrays):
             raise ValueError("N = %d rays but %s holds only %d" % (N, name, room))
 
 
+def _check_trace_operands(dtype, N, rows, ld, outputs, mask=None, path_sum=None):
+    """A trace writes rows x ld rays into each of Y, U, I (3 values per ray)
+    and T (1), N values of the rays' dtype into `path_sum` and ceil(N/32)
+    32-bit words into `mask`: refuse (ValueError, before anything is
+    launched) an operand of another element type or one too small for that."""
+    dtype = np.dtype(dtype)
+    _check_operands(dtype, N, path_sum=(path_sum, 1))
+    for name, (a, per_ray) in outputs.items():
+        if a is None:
+            continue
+        if np.dtype(a.dtype) != dtype:
+            raise ValueError("%s is %s but the rays are %s" % (name, np.dtype(a.dtype), dtype))
+        room = a.nbytes//(dtype.itemsize*per_ray)
+        if room < rows*ld:
+            raise ValueError("%s holds %d rays but %d rows of pitch %d need %d"
+                             % (name, room, rows, ld, rows*ld))
+    if mask is not None:
+        words = (N + 31)//32
+        if np.dtype(mask.dtype).itemsize != 4:
+            raise ValueError("mask must be 32-bit words, got %s" % np.dtype(mask.dtype))
+        if mask.nbytes//4 < words:
+            raise ValueError("N = %d rays need %d mask words but mask holds only %d"
+                             % (N, words, mask.nbytes//4))
+
+
 class DeviceArray:
     """A typed block of HBM owned by an Engine (freed with it or on .free())."""
 
@@ -260,7 +285,10 @@ class Engine:
         Asynchronous on the engine stream.  `mask`: optional uint32
         DeviceArray of ceil(N/32) words receiving the warp-ballot vignetting
         mask (bit set = the ray survives the last surface).  `path_sum`:
-        optional (N,) DeviceArray receiving sum_{s <= path_sum_upto} t[s]."""
+        optional (N,) DeviceArray receiving sum_{s <= path_sum_upto} t[s],
+        the left-to-right sum of the stored t.  Operands of another dtype
+        than the rays, or too small for rows x ld rays (N for path_sum,
+        ceil(N/32) words for mask), raise ValueError."""
         table = self._table(table)
         dt = _code(y0.dtype)
         N = y0.shape[0] if N is None else int(N)
@@ -271,6 +299,9 @@ class Engine:
         dp = lambda a: None if a is None else a.ptr  # noqa: E731
         if mask is None and path_sum is None and all(a is None for a in (Y, U, I, T)):
             raise ValueError("nothing to store: pass an output array, a mask or a path sum")
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
+        _check_trace_operands(y0.dtype, N, 1 if keep_last else len(table), int(ld),
+                              dict(Y=(Y, 3), U=(U, 3), I=(I, 3), T=(T, 1)), mask, path_sum)
         check(self.lib.rtx_set_mask_output(self.ctx, dp(mask)))
         check(self.lib.rtx_set_path_sum_output(self.ctx, dp(path_sum), int(path_sum_upto)))
         check(self.lib.rtx_trace(
@@ -292,6 +323,13 @@ class Engine:
         Ns = [a.shape[0] for a in y0s] if Ns is None else [int(n) for n in Ns]
         first = next(a for a in (Ys, Us, Is, Ts) if a is not None)[0]
         ld = first.shape[1] if ld is None else int(ld)
+        rows = 1 if keep_last else S
+        for b in range(nb):
+            pick = lambda xs: None if xs is None else xs[b]  # noqa: E731
+            _check_operands(y0s[0].dtype, Ns[b], y0=(y0s[b], 3), u0=(u0s[b], 3))
+            _check_trace_operands(y0s[0].dtype, Ns[b], rows, ld,
+                                  dict(Y=(pick(Ys), 3), U=(pick(Us), 3), I=(pick(Is), 3),
+                                       T=(pick(Ts), 1)))
         vp = C.c_void_p
 
         def arr(items, get):
@@ -379,14 +417,23 @@ class Engine:
         return [tuple(None if outs[k] is None else outs[k][b] for k in "yuit") for b in range(nb)]
 
     def trace_gather(self, table, y0, u0, dst_ptrs, dst_offset, N=None, clip=False,
-                     rot0=None, exact=False, dst_i_ptrs=None, xy=False):
+                     rot0=None, exact=False, dst_i_ptrs=None, xy=False, mask=None,
+                     path_sum=None, path_sum_upto=-1):
         """rtx_trace_gather: trace the local shard (DEVICE y0,u0) and store
         the last surface's intercepts into every buffer of `dst_ptrs` (raw
         device pointers: local or peer memory) at ray offset `dst_offset`;
         `dst_i_ptrs`: a second set of buffers for the incidence directions;
-        `xy`: the intercept buffers are (Ntotal, 2) and receive x,y only."""
+        `xy`: the intercept buffers are (Ntotal, 2) and receive x,y only.
+        `mask`, `path_sum`: the side outputs of trace_device for the shard's
+        N rays; without them both are switched off, so that a gather never
+        writes into buffers an earlier trace_device registered."""
         table = self._table(table)
         N = y0.shape[0] if N is None else int(N)
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
+        _check_trace_operands(y0.dtype, N, 1, N, {}, mask, path_sum)
+        dp = lambda a: None if a is None else a.ptr  # noqa: E731
+        check(self.lib.rtx_set_mask_output(self.ctx, dp(mask)))
+        check(self.lib.rtx_set_path_sum_output(self.ctx, dp(path_sum), int(path_sum_upto)))
         r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         arr = (C.c_void_p*len(dst_ptrs))(*[C.c_void_p(int(p)) for p in dst_ptrs])
         arr_i = None

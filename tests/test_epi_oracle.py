@@ -204,3 +204,49 @@ def test_engine_refuses_mismatched_operands():
         for k, call in enumerate(bad):
             with pytest.raises(ValueError):
                 call()
+
+
+def test_trace_device_refuses_mismatched_operands():
+    """Engine.trace_device, trace_device_batch and trace_gather: an output or
+    path sum of another dtype than the rays, an output smaller than rows x ld
+    rays, a path sum shorter than N or a mask that is not ceil(N/32) 32-bit
+    words raise ValueError before the library is called"""
+    from rayopt_b200.engine import Engine
+    eng = object.__new__(Engine)
+    eng.lib, eng.ctx = _NoLib(), None
+    table = load_golden("cooke_f07_clip")["table"]
+    S = len(table)
+    for dt, other in ((np.float32, np.float64), (np.float64, np.float32)):
+        y = _dev((100, 3), dt)
+        Y, T = _dev((S, 128, 3), dt), _dev((S, 128), dt)
+        bad = [
+            lambda: eng.trace_device(table, y, y, _dev((S, 128, 3), other), None, None, None),
+            lambda: eng.trace_device(table, y, y, None, None, None, _dev((S, 128), other), ld=128),
+            lambda: eng.trace_device(table, y, y, Y, _dev((S, 127, 3), dt), None, None, ld=128),
+            lambda: eng.trace_device(table, y, y, None, None, None, _dev((S - 1, 128), dt), ld=128),
+            lambda: eng.trace_device(table, y, y, _dev((1, 128, 3), dt), None, None, None),
+            lambda: eng.trace_device(table, y, y, Y, None, None, T, ld=256),
+            lambda: eng.trace_device(table, y, y, None, None, None, None, path_sum=_dev((100,), other)),
+            lambda: eng.trace_device(table, y, y, None, None, None, None, path_sum=_dev((99,), dt)),
+            lambda: eng.trace_device(table, y, y, None, None, None, None,
+                                     mask=_dev((4,), np.uint64)),
+            lambda: eng.trace_device(table, y, y, None, None, None, None,
+                                     mask=_dev((3,), np.uint32)),
+            lambda: eng.trace_device(table, y, _dev((100, 3), other), Y, None, None, None),
+            lambda: eng.trace_device(table, y, y, Y, None, None, None, N=129),
+            lambda: eng.trace_device_batch([table]*2, [y, y], [y, y], [Y, _dev((S, 128, 3), other)],
+                                           None, None, None),
+            lambda: eng.trace_device_batch([table]*2, [y, y], [y, y], [Y, _dev((S, 64, 3), dt)],
+                                           None, None, None, ld=128),
+            lambda: eng.trace_gather(table, y, y, [0x1000], 0, path_sum=_dev((100,), other)),
+            lambda: eng.trace_gather(table, y, y, [0x1000], 0, mask=_dev((3,), np.uint32)),
+        ]
+        for k, call in enumerate(bad):
+            with pytest.raises(ValueError):
+                call()
+        # operands that fit get through to the library
+        with pytest.raises(AssertionError, match="called"):
+            eng.trace_device(table, y, y, Y, None, None, T, mask=_dev((4,), np.uint32),
+                             path_sum=_dev((100,), dt))
+        with pytest.raises(AssertionError, match="called"):
+            eng.trace_device(table, y, y, _dev((1, 128, 3), dt), None, None, None, keep_last=True)
