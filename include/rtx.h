@@ -27,7 +27,14 @@
  * POSITIVE cudaError_t for CUDA failures.  Numerical failure (missed surface,
  * total internal reflection, vignetting, Newton non-convergence) is NOT an
  * error: it is NaN in the data, exactly where the reference puts it
- * (elements.py:208, 347-348, 367, 496).
+ * (elements.py:208, 347-348, 367, 496).  With RTX_EXACT that holds ray for
+ * ray on the decision boundaries too (aperture rim, tangent intercept,
+ * critical angle, Newton exits), with the reference's signs of zero and
+ * infinities.  The fast mode's NaN mask may differ within a few ulps of a
+ * boundary, never at the aperture rim when the intercept is the reference's
+ * own (tests/test_gpu_domain_edges.py).  Launch rays are expected to be
+ * finite: a NaN or infinite component gives NaN from that surface on where
+ * the reference has NaN or an infinity (the mask and counts agree).
  *
  * A context is bound to one GPU and one CUDA stream and is not thread-safe;
  * use one context per GPU (one process per GPU in multi-GPU runs).
@@ -344,6 +351,14 @@ int rtx_trace_gather(rtx_ctx *ctx, const rtx_surface *surf, int S,
  */
 int rtx_selftest_math(rtx_ctx *ctx, int64_t n, const double *a, const double *b,
                       double *out);
+/*
+ * The other primitives: for n host operand triples (a, b, c) writes 7*n
+ * doubles to `out` (host): a/b and c/b from the shared-reciprocal division of
+ * exact-mode refraction, a/b and c/b (IEEE __ddiv_rn), 1/b (the fast Newton
+ * step's reciprocal), sqrt(a) and 1/sqrt(a) (the fast Newton sag's pair).
+ */
+int rtx_selftest_math2(rtx_ctx *ctx, int64_t n, const double *a, const double *b,
+                       const double *c, double *out);
 
 /* ---- fused last-surface reductions (geometric_trace.py:171-183) ------- */
 /*

@@ -1498,6 +1498,35 @@ int rtx_selftest_math(rtx_ctx* ctx, int64_t n, const double* a, const double* b,
     return 0;
 }
 
+int rtx_selftest_math2(rtx_ctx* ctx, int64_t n, const double* a, const double* b,
+                       const double* c, double* out) {
+    if (!ctx || n < 1 || !a || !b || !c || !out) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    struct Bufs {  // freed on every return path
+        double *a = nullptr, *b = nullptr, *c = nullptr, *o = nullptr;
+        ~Bufs() {
+            cudaFree(a);
+            cudaFree(b);
+            cudaFree(c);
+            cudaFree(o);
+        }
+    } d;
+    CK(cudaMalloc((void**)&d.a, n * sizeof(double)));
+    CK(cudaMalloc((void**)&d.b, n * sizeof(double)));
+    CK(cudaMalloc((void**)&d.c, n * sizeof(double)));
+    CK(cudaMalloc((void**)&d.o, 7 * n * sizeof(double)));
+    CK(cudaMemcpyAsync(d.a, a, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d.b, b, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d.c, c, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    selftest_math2_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.a, d.b, d.c,
+                                                                               d.o, n);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, d.o, 7 * n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
 int rtx_moments(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* w,
                 const double* center, double* m) {
     if (!ctx || !y || !m || N < 0) return RTX_E_BADARG;

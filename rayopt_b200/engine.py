@@ -637,6 +637,16 @@ class Engine:
         check(self.lib.rtx_selftest_math(self.ctx, a.size, ptr(a), ptr(b), ptr(out)))
         return out
 
+    def selftest_math2(self, a, b, c):
+        """(7, n): shared-reciprocal a/b and c/b, IEEE a/b and c/b, fast 1/b,
+        fast sqrt(a) and 1/sqrt(a)"""
+        a, b, c = (np.ascontiguousarray(x, np.float64) for x in (a, b, c))
+        if not a.shape == b.shape == c.shape:
+            raise ValueError("a, b, c must have one shape")
+        out = np.empty((7, a.size))
+        check(self.lib.rtx_selftest_math2(self.ctx, a.size, ptr(a), ptr(b), ptr(c), ptr(out)))
+        return out
+
     def moments(self, y, w=None, N=None, center=None):
         """Weighted moments of device intercepts about `center`
         (include/rtx.h rtx_moments): 8 doubles."""

@@ -40,6 +40,15 @@ def test_abi_version_and_layout(lib):
     assert lib.rtx_sizeof_aim() == aim_dtype().itemsize     # struct rtx_aim
 
 
+def test_selftest_math2_rejects_bad_arguments(lib):
+    """the primitives' self-test entry point checks its arguments before any
+    device work (ABI version unchanged: a new symbol, no changed one)"""
+    a = np.ones(4)
+    p = a.ctypes.data_as(C.c_void_p)
+    assert lib.rtx_selftest_math2(None, 4, p, p, p, p) == -1         # RTX_E_BADARG
+    assert lib.rtx_abi_version() == 2
+
+
 def test_strerror(lib):
     assert b"bad argument" in lib.rtx_strerror(-1)
     assert lib.rtx_strerror(0) == b"ok"

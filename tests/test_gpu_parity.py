@@ -28,26 +28,50 @@ def _cmp(got, c, rtol, tag):
     return worst
 
 
+def _same_bits(a, b):
+    """bit patterns equal; any NaN matches any NaN"""
+    return (a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))
+
+
 def test_fp64_primitives(eng):
     """the kernels' branch-free FP64 division and sqrt are the IEEE results
-    (bit for bit) on normal-range operands, NaN/zero/negative included"""
+    bit for bit (signs of zero included) wherever operands and quotient are
+    normal or zero -- operands from 1e-8..1e8, near 2^+-1000, quotients near
+    the smallest normal and near overflow -- and for NaN operands and x/0.
+    Infinite operands are outside that domain (include/rtx.h)."""
     rng = np.random.default_rng(3)
     n = 1 << 20
     a = rng.standard_normal(n)*10.0**rng.integers(-8, 9, n)
     b = rng.standard_normal(n)*10.0**rng.integers(-8, 9, n)
-    a[:8] = [0., -0., np.nan, 1., -1., 4., 7., 2.]
-    b[:8] = [1., 2., 1., np.nan, 0., -0., 3., 0.]
+    m = n//8                                   # operands near 2^+-1000
+    a[:m] = rng.standard_normal(m)*2.0**rng.integers(-1000, 1001, m)
+    b[:m] = rng.standard_normal(m)*2.0**rng.integers(-1000, 1001, m)
+    a[m:2*m] = np.ldexp(1 + rng.random(m), -1000)            # quotient ~ 2^-1021
+    b[m:2*m] = np.ldexp(1 + rng.random(m), 21)*rng.choice([-1, 1], m)
+    a[2*m:3*m] = np.ldexp(1 + rng.random(m), 1000)           # quotient ~ 2^1023
+    b[2*m:3*m] = np.ldexp(1 + rng.random(m), -23)*rng.choice([-1, 1], m)
+    sp = [0., -0., np.nan, 1., -1., 4., 7., 2., np.inf, -np.inf]
+    pa, pb = np.meshgrid(sp, sp[:8] + [0., -0.])
+    a[3*m:3*m + pa.size], b[3*m:3*m + pa.size] = pa.ravel(), pb.ravel()
     out = eng.selftest_math(a, b)
-    # IEEE semantics for NaN operands and x/0 (infinite operands are outside
-    # the contract of the branch-free sequences and never occur on the path)
-    assert np.array_equal(out[0], out[1], equal_nan=True), "division"
-    assert np.array_equal(out[2], out[3], equal_nan=True), "sqrt"
-    fin = np.isfinite(a) & np.isfinite(b)
-    pos = fin & (a > 0)
-    np.testing.assert_allclose(out[4][pos], out[5][pos], rtol=4e-16)
     with np.errstate(all="ignore"):
-        assert np.array_equal(out[1][fin], (a/b)[fin], equal_nan=True)
-        assert np.array_equal(out[3][fin], np.sqrt(a)[fin], equal_nan=True)
+        q = a/b
+    tiny = np.finfo(np.float64).tiny
+    normal = lambda x: (np.abs(x) >= tiny) & np.isfinite(x)  # noqa: E731
+    ops = (normal(a) | (a == 0)) & normal(b) & np.isfinite(a) & (np.abs(b) < 2.**1022)
+    dom = (ops & (normal(q) | (q == 0))) | np.isnan(a) | np.isnan(b) | ((b == 0) & np.isfinite(a))
+    for cls, sel in (("2^+-1000", slice(0, m)), ("near the smallest normal", slice(m, 2*m)),
+                     ("near overflow", slice(2*m, 3*m)), ("specials", slice(3*m, 3*m + pa.size))):
+        print("division %s: %d of %d in the domain differ" % (
+            cls, (~_same_bits(out[0], out[1]) & dom)[sel].sum(), dom[sel].sum()))
+    assert _same_bits(out[0], out[1])[dom].all(), "division"
+    assert _same_bits(out[1], q)[dom].all(), "__ddiv_rn vs numpy"
+    sq = np.isnan(a) | (a == 0) | (a < 0) | normal(a)
+    assert _same_bits(out[2], out[3])[sq & np.isfinite(a)].all(), "sqrt"
+    with np.errstate(all="ignore"):
+        assert _same_bits(out[3], np.sqrt(a))[sq & np.isfinite(a)].all()
+    pos = normal(a) & (a > 0)
+    np.testing.assert_allclose(out[4][pos], out[5][pos], rtol=4e-16)
 
 
 @pytest.mark.parametrize("rpt", [1, 2])
