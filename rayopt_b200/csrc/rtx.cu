@@ -51,6 +51,20 @@ struct ChunkBuf {
     cudaStream_t stream = nullptr;
 };
 
+// the RTX_* environment knobs (rtx_init): experiments that override the
+// per-call choice of choose_trace_cfg
+struct Tuning {
+    bool tuned = false;       // RTX_RPT / RTX_STORE / RTX_WARPS / RTX_NBUF / RTX_CLUSTER was set
+    int rpt = 2;              // rays per thread
+    int store = STORE_CTA;    // STORE_WARP / STORE_CTA
+    int warps = 16;           // warps per CTA
+    int nbuf = 1;             // staging buffers per CTA
+    int cluster = 1;          // CTAs per cluster of the per-CTA store kernel
+    int lockstep = 1;         // CTA barrier per stored surface (STORE_WARP)
+    int max_ctas_per_sm = 0;  // 0: whatever fits
+    int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
+};
+
 }  // namespace
 
 struct rtx_ctx {
@@ -79,15 +93,8 @@ struct rtx_ctx {
     size_t small_bytes = 0;
     int64_t launches = 0;
     int max_smem_optin = 0;
-    // kernel configuration (defaults; trace_device picks per call)
-    int default_rpt = 2;      // rays per thread
-    int store = 2;            // STORE_WARP / STORE_CTA
-    int warps = 16;           // warps per CTA
-    int nbuf = 1;             // staging buffers per CTA
-    int lockstep = 1;         // CTA barrier per stored surface (STORE_WARP)
-    int cluster = 1;          // CTAs per cluster of the per-CTA store kernel (RTX_CLUSTER)
-    int max_ctas_per_sm = 0;  // 0: whatever fits
-    int last_ctas = 0;        // CTAs of the last trace launch (rtx_last_launch_ctas)
+    Tuning tuning;
+    int last_ctas = 0;  // CTAs of the last trace launch (rtx_last_launch_ctas)
     int last_cfg[5] = {0, 0, 0, 0, 0};  // rpt, store, warps, nbuf, cluster (rtx_last_launch_config)
     unsigned* mask = nullptr; // rtx_set_mask_output
     void* tsum = nullptr;     // rtx_set_path_sum_output
@@ -95,8 +102,6 @@ struct rtx_ctx {
     // rtx_numa_bind: what to restore
     bool numa_bound = false;
     cpu_set_t saved_affinity;
-    bool tuned = false;       // an RTX_* environment knob overrides the heuristics
-    int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
     // rtx_grid_linear: claim grid when the caller wants no winner output
     int* d_winner = nullptr;
     size_t winner_cap = 0;
@@ -187,14 +192,15 @@ template <typename T, bool EXACT, int RPT, int STORE, int WARPS, int NBUF, int C
 int launch_one(rtx_ctx* ctx, const TraceParams<T>& p, cudaStream_t stream) {
     auto kern = trace_kernel<T, EXACT, RPT, STORE, WARPS, NBUF, CLUSTER>;
     constexpr int threads = WARPS * 32;
-    size_t smem = trace_smem_bytes<T, RPT>(p.S, STORE, WARPS, NBUF);
+    size_t smem = trace_smem_bytes(sizeof(T), p.S, RPT, STORE, WARPS, NBUF);
     if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
     if (smem > 48 * 1024)
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
     if (occ < 1) occ = 1;
-    if (ctx->max_ctas_per_sm > 0 && occ > ctx->max_ctas_per_sm) occ = ctx->max_ctas_per_sm;
+    const int max_ctas = ctx->tuning.max_ctas_per_sm;
+    if (max_ctas > 0 && occ > max_ctas) occ = max_ctas;
     const long long per_cta = (long long)threads * RPT;
     TraceParams<T> q = p;  // launch-wide CTA-tile numbering over the bundles
     long long tiles = 0;
@@ -245,89 +251,79 @@ int launch_one(rtx_ctx* ctx, const TraceParams<T>& p, cudaStream_t stream) {
     return (int)cudaGetLastError();
 }
 
-// the instantiated tuning space (rpt, store, warps, nbuf, cluster)
-template <typename T, bool EXACT>
-int launch_cfg(rtx_ctx* ctx, const TraceParams<T>& p, int rpt, int store, int warps, int nbuf,
-               int cluster, cudaStream_t stream) {
-#define RTX_CASE(R, ST, W, NB)                                  \
-    if (rpt == R && store == ST && warps == W && nbuf == NB)    \
-        return launch_one<T, EXACT, R, ST, W, NB>(ctx, p, stream);
-#define RTX_CLUSTER_CASE(R, W, NB, CL)                                               \
-    if (rpt == R && store == STORE_CTA && warps == W && nbuf == NB && cluster == CL) \
-        return launch_one<T, EXACT, R, STORE_CTA, W, NB, CL>(ctx, p, stream);
-    if (store == STORE_DIRECT) return launch_one<T, EXACT, 1, STORE_DIRECT, 8, 1>(ctx, p, stream);
-    // clusters: single-bundle per-CTA stores only (batched launches, fused
-    // gathers and keep-LAST traces keep the per-CTA kernel)
-    if (cluster > 1 && store == STORE_CTA && p.nbatch == 1 && p.npeer == 0 && !p.keep_last) {
-        if constexpr (sizeof(T) == 8) {
-            RTX_CLUSTER_CASE(2, 16, 1, DEFAULT_CLUSTER)
-        }
-#ifdef RTX_TUNING_SPACE
-        if constexpr (sizeof(T) == 8) {
-            RTX_CLUSTER_CASE(2, 16, 1, 2)
-            RTX_CLUSTER_CASE(2, 16, 1, 4)
-            RTX_CLUSTER_CASE(2, 16, 1, 8)
-        } else {
-            RTX_CLUSTER_CASE(4, 16, 1, 2)
-            RTX_CLUSTER_CASE(4, 16, 1, 4)
-            RTX_CLUSTER_CASE(4, 16, 1, 8)
-            RTX_CLUSTER_CASE(4, 16, 1, 16)
-        }
-#endif
-        return RTX_E_UNSUPPORTED;
-    }
-    RTX_CASE(1, STORE_WARP, 8, 2)
-    RTX_CASE(2, STORE_WARP, 8, 2)
-    RTX_CASE(2, STORE_CTA, 16, 1)
-    RTX_CASE(1, STORE_CTA, 16, 1)
-    RTX_CASE(2, STORE_CTA, 32, 1)
-    RTX_CASE(2, STORE_CTA, 8, 1)
-    RTX_CASE(2, STORE_WARP, 16, 2)
-    if constexpr (sizeof(T) == 4) {  // FP32: four rays per thread (64 registers leave room)
-        RTX_CASE(4, STORE_CTA, 16, 1)
-        RTX_CASE(4, STORE_WARP, 16, 1)
-    }
-#ifdef RTX_TUNING_SPACE
-    RTX_CASE(2, STORE_CTA, 8, 2)
-    RTX_CASE(1, STORE_WARP, 16, 2)
-    RTX_CASE(2, STORE_WARP, 8, 1)
-    RTX_CASE(1, STORE_CTA, 8, 1)
-    RTX_CASE(1, STORE_CTA, 8, 2)
-    RTX_CASE(1, STORE_CTA, 16, 2)
-    RTX_CASE(2, STORE_CTA, 16, 2)
-    RTX_CASE(1, STORE_CTA, 32, 1)
-    RTX_CASE(1, STORE_CTA, 32, 2)
-    if constexpr (sizeof(T) == 4) {
-        RTX_CASE(4, STORE_WARP, 8, 1)
-        RTX_CASE(4, STORE_CTA, 8, 1)
-        RTX_CASE(4, STORE_CTA, 32, 1)
-    }
-    RTX_CASE(2, STORE_WARP, 16, 1)
-    if constexpr (sizeof(T) == 4) {
-        RTX_CASE(4, STORE_WARP, 16, 2)
-        RTX_CASE(4, STORE_WARP, 8, 2)
-    }
-#endif
-#undef RTX_CLUSTER_CASE
-#undef RTX_CASE
-    return RTX_E_UNSUPPORTED;
-}
+struct TraceCfg {
+    int rpt, store, warps, nbuf, cluster, lockstep;
+};
 
+// One row of the instantiated tuning space.  ONLY: the element size of the
+// one arithmetic type the kernel is built for (0: both); in the other type's
+// table the row is empty.
 template <typename T>
-int launch_trace(rtx_ctx* ctx, const TraceParams<T>& p, bool exact, int rpt, int store, int warps,
-                 int nbuf, int cluster, cudaStream_t stream);
+struct KernelRow {
+    int rpt, store, warps, nbuf, cluster;
+    int (*launch)(rtx_ctx*, const TraceParams<T>&, cudaStream_t);
+};
 
-template <>
-int launch_trace<double>(rtx_ctx* ctx, const TraceParams<double>& p, bool exact, int rpt,
-                         int store, int warps, int nbuf, int cluster, cudaStream_t stream) {
-    if (exact) return launch_cfg<double, true>(ctx, p, rpt, store, warps, nbuf, cluster, stream);
-    return launch_cfg<double, false>(ctx, p, rpt, store, warps, nbuf, cluster, stream);
+template <typename T, bool EXACT, int RPT, int STORE, int WARPS, int NBUF, int CLUSTER = 1,
+          int ONLY = 0>
+constexpr KernelRow<T> row() {
+    if constexpr (ONLY != 0 && ONLY != (int)sizeof(T))
+        return {0, 0, 0, 0, 0, nullptr};
+    else
+        return {RPT, STORE, WARPS, NBUF, CLUSTER,
+                &launch_one<T, EXACT, RPT, STORE, WARPS, NBUF, CLUSTER>};
 }
-template <>
-int launch_trace<float>(rtx_ctx* ctx, const TraceParams<float>& p, bool exact, int rpt, int store,
-                        int warps, int nbuf, int cluster, cudaStream_t stream) {
-    if (exact) return RTX_E_UNSUPPORTED;  // RTX_EXACT is FP64 only
-    return launch_cfg<float, false>(ctx, p, rpt, store, warps, nbuf, cluster, stream);
+
+constexpr int F32 = 4, F64 = 8;
+
+template <typename T, bool EXACT>
+constexpr KernelRow<T> KERNELS[] = {
+    row<T, EXACT, 1, STORE_DIRECT, 8, 1>(),
+    row<T, EXACT, 1, STORE_WARP, 8, 2>(),
+    row<T, EXACT, 2, STORE_WARP, 8, 2>(),
+    row<T, EXACT, 2, STORE_CTA, 16, 1>(),
+    row<T, EXACT, 1, STORE_CTA, 16, 1>(),
+    row<T, EXACT, 2, STORE_CTA, 32, 1>(),
+    row<T, EXACT, 2, STORE_CTA, 8, 1>(),
+    row<T, EXACT, 2, STORE_WARP, 16, 2>(),
+    // FP32: four rays per thread (64 registers leave room)
+    row<T, EXACT, 4, STORE_CTA, 16, 1, 1, F32>(),
+    row<T, EXACT, 4, STORE_WARP, 16, 1, 1, F32>(),
+    // FP64: clusters of per-CTA stores (FP32 clusters only in the tuning space)
+    row<T, EXACT, 2, STORE_CTA, 16, 1, DEFAULT_CLUSTER, F64>(),
+#ifdef RTX_TUNING_SPACE
+    row<T, EXACT, 2, STORE_CTA, 16, 1, 2, F64>(),
+    row<T, EXACT, 2, STORE_CTA, 16, 1, 4, F64>(),
+    row<T, EXACT, 2, STORE_CTA, 16, 1, 8, F64>(),
+    row<T, EXACT, 4, STORE_CTA, 16, 1, 2, F32>(),
+    row<T, EXACT, 4, STORE_CTA, 16, 1, 4, F32>(),
+    row<T, EXACT, 4, STORE_CTA, 16, 1, 8, F32>(),
+    row<T, EXACT, 4, STORE_CTA, 16, 1, 16, F32>(),
+    row<T, EXACT, 2, STORE_CTA, 8, 2>(),
+    row<T, EXACT, 1, STORE_WARP, 16, 2>(),
+    row<T, EXACT, 2, STORE_WARP, 8, 1>(),
+    row<T, EXACT, 1, STORE_CTA, 8, 1>(),
+    row<T, EXACT, 1, STORE_CTA, 8, 2>(),
+    row<T, EXACT, 1, STORE_CTA, 16, 2>(),
+    row<T, EXACT, 2, STORE_CTA, 16, 2>(),
+    row<T, EXACT, 1, STORE_CTA, 32, 1>(),
+    row<T, EXACT, 1, STORE_CTA, 32, 2>(),
+    row<T, EXACT, 4, STORE_WARP, 8, 1, 1, F32>(),
+    row<T, EXACT, 4, STORE_CTA, 8, 1, 1, F32>(),
+    row<T, EXACT, 4, STORE_CTA, 32, 1, 1, F32>(),
+    row<T, EXACT, 2, STORE_WARP, 16, 1>(),
+    row<T, EXACT, 4, STORE_WARP, 16, 2, 1, F32>(),
+    row<T, EXACT, 4, STORE_WARP, 8, 2, 1, F32>(),
+#endif
+};
+
+template <typename T, bool EXACT>
+int launch_kernel(rtx_ctx* ctx, const TraceParams<T>& p, const TraceCfg& c, cudaStream_t stream) {
+    for (const KernelRow<T>& k : KERNELS<T, EXACT>)
+        if (k.launch && k.rpt == c.rpt && k.store == c.store && k.warps == c.warps &&
+            k.nbuf == c.nbuf && k.cluster == c.cluster)
+            return k.launch(ctx, p, stream);
+    return RTX_E_UNSUPPORTED;
 }
 
 // convert + upload the table; returns the device pointer.  The copy is
@@ -383,11 +379,10 @@ int check_table(const rtx_surface* surf, int S) {
     return 0;
 }
 
-template <typename T>
-struct Batch {
-    int n = 0;
-    BatchItem<T> item[RTX_MAX_BATCH];
-};
+bool valid_keep_dtype(int keep, int dtype) {
+    return (keep == RTX_KEEP_ALL || keep == RTX_KEEP_LAST) &&
+           (dtype == RTX_F64 || dtype == RTX_F32);
+}
 
 struct PeerDst {
     int n = 0;
@@ -398,202 +393,217 @@ struct PeerDst {
     bool xy = false;
 };
 
+// One trace launch as a front end describes it: the common part, 1 to
+// RTX_MAX_BATCH bundles (each with its uploaded table) and, for a single
+// bundle, the gather destinations and the per-ray side outputs.
 template <typename T>
-int trace_device(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, long long N,
-                 const void* y0, const void* u0, int clip, int keep, long long ld, void* Y,
-                 void* U, void* I, void* Tt, unsigned flags, cudaStream_t stream,
-                 const DevSurf<T>* table /* may be null: upload */,
-                 const PeerDst* peers = nullptr, const Batch<T>* batch = nullptr) {
-    if (!table) {
-        int rc = upload_table<T>(ctx, surf, S, stream, &table);
-        if (rc) return rc;
+struct Launch {
+    int S;
+    int clip;
+    bool keep_last;
+    const double* rot0;
+    long long ld;
+    unsigned flags;  // RTX_EXACT, RTX_STORE_DIRECT, RTX_RPT1 / RTX_RPT2
+    int newton = 0;  // Newton surfaces of the first bundle's table
+    int n = 0;
+    BatchItem<T> item[RTX_MAX_BATCH];
+    const PeerDst* peers = nullptr;
+    unsigned* mask = nullptr;
+    T* tsum = nullptr;
+    int tsum_upto = 0;
+
+    Launch(const rtx_surface* surf, int S_, const double* rot0_, int clip_, int keep,
+           long long ld_, unsigned flags_)
+        : S(S_), clip(clip_ ? 1 : 0), keep_last(keep == RTX_KEEP_LAST), rot0(rot0_), ld(ld_),
+          flags(flags_) {
+        for (int i = 0; i < S; ++i) newton += surf[i].n_asph >= 0;
     }
-    TraceParams<T> p;
-    memset(&p, 0, sizeof(p));
-    p.lockstep = 0;
-    p.table = table;
-    p.S = S;
-    p.clip = clip ? 1 : 0;
-    p.keep_last = keep == RTX_KEEP_LAST;
-    p.has_rot0 = rot0 != nullptr;
-    if (rot0)
-        for (int i = 0; i < 9; ++i) p.rot0[i] = (T)rot0[i];
-    p.N = N;
-    p.ld = ld;
-    p.y0 = (const T*)y0;
-    p.u0 = (const T*)u0;
-    p.Y = (T*)Y;
-    p.U = (T*)U;
-    p.I = (T*)I;
-    p.Tt = (T*)Tt;
-    bool peers_ok = true;
-    if (peers && peers->n > 0) {
-        p.npeer = peers->n;
-        p.peer_off = peers->off;
-        p.peer_has_i = peers->has_i ? 1 : 0;
-        p.peer_xy = peers->xy ? 1 : 0;
-        for (int k = 0; k < peers->n; ++k) {
-            p.peer[k] = (T*)peers->ptr[k];
-            p.peer_i[k] = (T*)peers->ptr_i[k];
-        }
-        // bulk stores need 16-byte aligned runs in every destination
-        peers_ok = (peers->off * (peers->xy ? 2 : 3) * (long long)sizeof(T)) % 16 == 0 &&
-                   (!peers->has_i || (peers->off * 3 * (long long)sizeof(T)) % 16 == 0);
-        for (int k = 0; k < peers->n; ++k) {
-            peers_ok = peers_ok && (reinterpret_cast<uintptr_t>(peers->ptr[k]) & 15u) == 0;
-            peers_ok = peers_ok && (reinterpret_cast<uintptr_t>(peers->ptr_i[k]) & 15u) == 0;
-        }
+    void add(const DevSurf<T>* table, long long N, const void* y0, const void* u0, void* Y,
+             void* U, void* I, void* Tt) {
+        item[n++] = {table, (const T*)y0, (const T*)u0, (T*)Y, (T*)U, (T*)I, (T*)Tt, N, 0};
     }
-    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
-    int rpt = ctx->default_rpt;
-    if (flags & RTX_RPT1) rpt = 1;
-    if (flags & RTX_RPT2) rpt = 2;
-    int store = ctx->store, warps = ctx->warps, nbuf = ctx->nbuf;
-    bool heavy = false;
-    const bool explicit_rpt = (flags & (RTX_RPT1 | RTX_RPT2)) != 0;
-    if (!ctx->tuned && !explicit_rpt) {
-        // configurations by workload (scripts/sweep.py compares them):
-        //  FP64: 2 rays/thread x 16 warps, per-CTA bulk stores (24 KB runs)
-        //  FP32: 4 rays/thread x 16 warps (2048-ray tiles, 24 KB runs again):
-        //        half the per-thread overhead instructions of 2 rays/thread
-        //  systems with >= 25 % Newton (aspheric) surfaces are bound by issue
-        //  slots / the FP64 pipe, not by HBM: free-running 16-warp CTAs with
-        //  per-warp stores (no lockstep barrier behind the long, divergent
-        //  Newton chains)
-        int newton = 0;
-        for (int i = 0; i < S; ++i) newton += surf && surf[i].n_asph >= 0;
-        // ... and so is a keep-LAST trace (one stored row: the stores are no
-        // limit): free-running CTAs
-        // (a fused gather keeps the per-CTA 24 KB runs for its NVLink stores)
-        heavy = newton * 4 >= S || (keep == RTX_KEEP_LAST && !(peers && peers->n > 0));
-        if (sizeof(T) == 4) {
-            rpt = 4;
-            if (heavy) {
-                store = STORE_WARP;
-                warps = 16;
-                nbuf = 1;
-            } else {
-                store = STORE_CTA;
-                warps = 16;
-                nbuf = 1;
-            }
-        } else if (heavy) {
-            // free-running 16-warp CTAs with per-warp stores
-            rpt = 2;
-            store = STORE_WARP;
-            nbuf = 2;
-            warps = 16;
-        }
-    }
+};
+
+// what the kernel configuration depends on
+struct TraceShape {
+    size_t elem;     // sizeof(T)
+    int S;
+    int newton;      // Newton surfaces of the first bundle's table
+    long long N;     // the largest bundle
+    long long ld;
+    bool keep_last;
+    int nbatch;
+    bool gather;
+    bool aligned;    // every output and peer destination 16-byte aligned
+    unsigned flags;  // RTX_STORE_DIRECT, RTX_RPT1 / RTX_RPT2
+};
+
+// The kernel configuration of a launch (DESIGN.md 3.2): the library's own
+// choice by workload, or the RTX_* knobs of an experiment (tu.tuned).
+TraceCfg choose_trace_cfg(const TraceShape& sh, const Tuning& tu, size_t smem_optin) {
+    const bool explicit_rpt = (sh.flags & (RTX_RPT1 | RTX_RPT2)) != 0;
+    const bool fp32 = sh.elem == 4;
+    const bool own = !tu.tuned && !explicit_rpt;  // configurations by workload
+    // Systems with >= 25 % Newton (aspheric) surfaces are bound by issue slots
+    // / the FP64 pipe, not by HBM, and so is a keep-LAST trace (one stored
+    // row: the stores are no limit): free-running CTAs with per-warp stores,
+    // no lockstep barrier behind the long, divergent Newton chains.  (A fused
+    // gather keeps the per-CTA 24 KB runs for its NVLink stores.)
+    const bool heavy = own && (sh.newton * 4 >= sh.S || (sh.keep_last && !sh.gather));
+    TraceCfg c = {tu.rpt, tu.store, tu.warps, tu.nbuf, tu.cluster, heavy ? 0 : tu.lockstep};
+    auto set = [&c](int rpt, int store, int warps, int nbuf) {
+        c.rpt = rpt;
+        c.store = store;
+        c.warps = warps;
+        c.nbuf = nbuf;
+    };
+    if (sh.flags & RTX_RPT1) c.rpt = 1;
+    if (sh.flags & RTX_RPT2) c.rpt = 2;
+    //  FP64: 2 rays/thread x 16 warps, per-CTA bulk stores (24 KB runs)
+    //  FP32: 4 rays/thread x 16 warps (2048-ray tiles, 24 KB runs again):
+    //        half the per-thread overhead instructions of 2 rays/thread
+    if (own && fp32) set(4, heavy ? STORE_WARP : STORE_CTA, 16, 1);
+    else if (heavy) set(2, STORE_WARP, 16, 2);
     // (an explicit RPT request is honoured at every N; the pitch and alignment
     // step-downs below still apply to it)
-    if (N <= 150 * 1000 && !ctx->tuned && !explicit_rpt) {
-        // small bundles: 256-ray warp tiles spread over all SMs
-        rpt = 1;
-        store = STORE_WARP;
-        warps = 8;
-        nbuf = 2;
-    } else if (N <= 1500 * 1000 && !ctx->tuned && !explicit_rpt && !heavy && sizeof(T) == 8) {
+    if (own && sh.N <= 150 * 1000) {
+        set(1, STORE_WARP, 8, 2);  // small bundles: 256-ray warp tiles spread over all SMs
+    } else if (own && !heavy && !fp32 && sh.N <= 1500 * 1000) {
         // mid-size FP64 bundles (what an analysis traces): 512-ray tiles, two
         // resident CTAs per SM -- twice the tiles to balance over the SMs
-        rpt = 1;
-        store = STORE_CTA;
-        warps = 16;
-        nbuf = 1;
-    } else if (N > 500 * 1000 && N <= 2500 * 1000 && !ctx->tuned && !explicit_rpt && !heavy &&
-               sizeof(T) == 4) {
-        // mid-size FP32 bundles: 512-ray tiles, three resident CTAs per SM
-        rpt = 2;
-        store = STORE_CTA;
-        warps = 8;
-        nbuf = 1;
-    } else if (N <= 32 * 1024 && !explicit_rpt) {  // (tuned contexts keep the old small-bundle rule)
-        rpt = 1;
-        store = STORE_WARP;
-        warps = 8;
-        nbuf = 2;
+        set(1, STORE_CTA, 16, 1);
+    } else if (own && !heavy && fp32 && sh.N > 500 * 1000 && sh.N <= 2500 * 1000) {
+        set(2, STORE_CTA, 8, 1);  // mid-size FP32 bundles: 512-ray tiles, three CTAs per SM
+    } else if (!explicit_rpt && sh.N <= 32 * 1024) {
+        set(1, STORE_WARP, 8, 2);  // (tuned contexts keep the old small-bundle rule)
     } else if (explicit_rpt) {  // explicit RPT: its per-warp store kernel
-        store = STORE_WARP;
-        warps = 8;
-        nbuf = 2;
+        set(c.rpt, STORE_WARP, 8, 2);
     }
-    const bool aligned = !(flags & RTX_STORE_DIRECT) && al16(Y) && al16(U) && al16(I) && al16(Tt) &&
-                         peers_ok;
     // The staged paths write whole 32*rpt-ray groups: the pitch must be a
     // multiple of that, and so must the shard of a gather (into a gather buffer
     // a ragged tail would spill clamped copies of the last ray into the next
     // rank's range -- a race with that rank's own stores).
-    auto fits = [&](int r) { return ld % (32 * r) == 0 && (p.npeer == 0 || N % (32 * r) == 0); };
-    if (aligned && !ctx->tuned) {
+    const bool aligned = sh.aligned && !(sh.flags & RTX_STORE_DIRECT);
+    auto fits = [&sh](int r) {
+        return sh.ld % (32 * r) == 0 && (!sh.gather || sh.N % (32 * r) == 0);
+    };
+    if (aligned && !tu.tuned) {
         // step down to the kernel with fewer rays per thread that fits
-        if (rpt == 4 && !fits(4)) {
-            rpt = 2;
-            if (heavy) {
-                store = STORE_WARP;
-                warps = 8;
-                nbuf = 2;
-            } else {
-                store = STORE_CTA;
-                warps = 32;
-                nbuf = 1;
-            }
+        if (c.rpt == 4 && !fits(4)) {
+            if (heavy)
+                set(2, STORE_WARP, 8, 2);
+            else
+                set(2, STORE_CTA, 32, 1);
         }
-        if (rpt == 2 && !fits(2) && fits(1)) {
-            rpt = 1;
-            store = STORE_WARP;
-            warps = 8;
-            nbuf = 2;
-        }
+        if (c.rpt == 2 && !fits(2) && fits(1)) set(1, STORE_WARP, 8, 2);
     }
-    if (!(aligned && fits(rpt))) store = STORE_DIRECT;  // per-ray stores: exactly N rays
+    if (!(aligned && fits(c.rpt))) c.store = STORE_DIRECT;  // per-ray stores: exactly N rays
     // a long table leaves less shared memory for the staging buffers (256 FP64
     // surfaces take 92 KB): step down to the smallest staged kernel, then to
     // per-ray stores, rather than refuse a table the library accepts
-    auto smem_of = [&](int r, int st, int w, int nb) {
-        return r == 4 ? trace_smem_bytes<T, 4>(S, st, w, nb)
-                      : r == 2 ? trace_smem_bytes<T, 2>(S, st, w, nb)
-                               : trace_smem_bytes<T, 1>(S, st, w, nb);
+    auto smem = [&sh](int rpt, int store, int warps, int nbuf) {
+        return trace_smem_bytes(sh.elem, sh.S, rpt, store, warps, nbuf);
     };
-    const size_t optin = (size_t)ctx->max_smem_optin;
-    if (!ctx->tuned && store != STORE_DIRECT && smem_of(rpt, store, warps, nbuf) > optin) {
-        if (fits(1) && smem_of(1, STORE_WARP, 8, 2) <= optin) {
-            rpt = 1;
-            store = STORE_WARP;
-            warps = 8;
-            nbuf = 2;
-        } else {
-            store = STORE_DIRECT;
-        }
+    if (!tu.tuned && c.store != STORE_DIRECT &&
+        smem(c.rpt, c.store, c.warps, c.nbuf) > smem_optin) {
+        if (fits(1) && smem(1, STORE_WARP, 8, 2) <= smem_optin)
+            set(1, STORE_WARP, 8, 2);
+        else
+            c.store = STORE_DIRECT;
     }
-    if (batch && batch->n > 0) {
-        p.nbatch = batch->n;
-        for (int b = 0; b < batch->n; ++b) p.item[b] = batch->item[b];
-    } else {
-        p.nbatch = 1;
-        p.item[0].table = table;
-        p.item[0].y0 = p.y0;
-        p.item[0].u0 = p.u0;
-        p.item[0].Y = p.Y;
-        p.item[0].U = p.U;
-        p.item[0].I = p.I;
-        p.item[0].Tt = p.Tt;
-        p.item[0].N = N;
-    }
-    p.lockstep = heavy ? 0 : ctx->lockstep;
-    p.tune = ctx->tune;
-    p.mask = ctx->mask;
-    p.tsum = (T*)ctx->tsum;
-    p.tsum_upto = ctx->tsum_upto < 0 ? S - 1 : ctx->tsum_upto;
     // large FP64 analytic bundles: clusters of CTAs whose stores leave as one
     // run (DEFAULT_CLUSTER).  FP32 stays unclustered: 8-CTA clusters gained
-    // only 3-4 % there (1.77-1.78 vs 1.84 ms, C2 in FP32).  launch_cfg keeps
-    // batched launches, gathers and keep-LAST traces on the per-CTA kernel.
-    int cluster = ctx->cluster;
-    if (!ctx->tuned && !explicit_rpt && !heavy && sizeof(T) == 8 && N > 1500 * 1000 &&
-        store == STORE_CTA && rpt == 2 && warps == 16 && nbuf == 1)
-        cluster = DEFAULT_CLUSTER;
-    return launch_trace<T>(ctx, p, (flags & RTX_EXACT) != 0, rpt, store, warps, nbuf, cluster,
-                           stream);
+    // only 3-4 % there (1.77-1.78 vs 1.84 ms, C2 in FP32).
+    if (own && !heavy && !fp32 && sh.N > 1500 * 1000 && c.rpt == 2 && c.store == STORE_CTA &&
+        c.warps == 16 && c.nbuf == 1)
+        c.cluster = DEFAULT_CLUSTER;
+    // clusters: single-bundle keep-ALL per-CTA stores only (batched launches,
+    // fused gathers and keep-LAST traces keep the per-CTA kernel)
+    if (sh.nbatch != 1 || sh.gather || sh.keep_last || c.store != STORE_CTA) c.cluster = 1;
+    if (c.store == STORE_DIRECT) set(1, STORE_DIRECT, 8, 1);
+    return c;
+}
+
+bool al16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; }
+
+template <typename T>
+TraceShape shape_of(const Launch<T>& L) {
+    TraceShape sh = {sizeof(T), L.S, L.newton, 0, L.ld, L.keep_last, L.n, L.peers != nullptr,
+                     true, L.flags};
+    for (int b = 0; b < L.n; ++b) {
+        const BatchItem<T>& it = L.item[b];
+        sh.N = it.N > sh.N ? it.N : sh.N;
+        sh.aligned = sh.aligned && al16(it.Y) && al16(it.U) && al16(it.I) && al16(it.Tt);
+    }
+    if (const PeerDst* pd = L.peers) {
+        // bulk stores need 16-byte aligned runs in every destination
+        sh.aligned = sh.aligned && (pd->off * (pd->xy ? 2 : 3) * (long long)sizeof(T)) % 16 == 0 &&
+                     (!pd->has_i || (pd->off * 3 * (long long)sizeof(T)) % 16 == 0);
+        for (int k = 0; k < pd->n; ++k)
+            sh.aligned = sh.aligned && al16(pd->ptr[k]) && al16(pd->ptr_i[k]);
+    }
+    return sh;
+}
+
+template <typename T>
+int launch_trace(rtx_ctx* ctx, const Launch<T>& L, cudaStream_t stream) {
+    const TraceCfg c = choose_trace_cfg(shape_of(L), ctx->tuning, (size_t)ctx->max_smem_optin);
+    TraceParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.S = L.S;
+    p.clip = L.clip;
+    p.keep_last = L.keep_last;
+    p.has_rot0 = L.rot0 != nullptr;
+    if (L.rot0)
+        for (int i = 0; i < 9; ++i) p.rot0[i] = (T)L.rot0[i];
+    p.ld = L.ld;
+    p.lockstep = c.lockstep;
+    p.tune = ctx->tuning.tune;
+    if (const PeerDst* pd = L.peers) {
+        p.npeer = pd->n;
+        p.peer_off = pd->off;
+        p.peer_has_i = pd->has_i ? 1 : 0;
+        p.peer_xy = pd->xy ? 1 : 0;
+        for (int k = 0; k < pd->n; ++k) {
+            p.peer[k] = (T*)pd->ptr[k];
+            p.peer_i[k] = (T*)pd->ptr_i[k];
+        }
+    }
+    p.mask = L.mask;
+    p.tsum = L.tsum;
+    p.tsum_upto = L.tsum_upto < 0 ? L.S - 1 : L.tsum_upto;
+    p.nbatch = L.n;
+    for (int b = 0; b < L.n; ++b) p.item[b] = L.item[b];
+    if (L.flags & RTX_EXACT) {
+        if constexpr (sizeof(T) == 8) return launch_kernel<T, true>(ctx, p, c, stream);
+        return RTX_E_UNSUPPORTED;  // RTX_EXACT is FP64 only
+    }
+    return launch_kernel<T, false>(ctx, p, c, stream);
+}
+
+// upload the table of a new bundle of `L` (on the context stream, keeping the
+// tables of the bundles before it) and add the bundle
+template <typename T>
+int add_bundle(rtx_ctx* ctx, Launch<T>& L, const rtx_surface* surf, long long N, const void* y0,
+               const void* u0, void* Y, void* U, void* I, void* Tt) {
+    const void* keep[RTX_MAX_BATCH];
+    for (int b = 0; b < L.n; ++b) keep[b] = L.item[b].table;
+    const DevSurf<T>* table = nullptr;
+    int rc = upload_table<T>(ctx, surf, L.S, ctx->stream, &table, keep, L.n);
+    if (rc) return rc;
+    L.add(table, N, y0, u0, Y, U, I, Tt);
+    return 0;
+}
+
+// rtx_trace, rtx_trace_gather: one bundle with the registered side outputs
+template <typename T>
+int trace_registered(rtx_ctx* ctx, Launch<T>& L, const rtx_surface* surf, long long N,
+                     const void* y0, const void* u0, void* Y, void* U, void* I, void* Tt) {
+    L.mask = ctx->mask;
+    L.tsum = (T*)ctx->tsum;
+    L.tsum_upto = ctx->tsum_upto;
+    int rc = add_bundle<T>(ctx, L, surf, N, y0, u0, Y, U, I, Tt);
+    return rc ? rc : launch_trace<T>(ctx, L, ctx->stream);
 }
 
 int ensure_chunk(rtx_ctx* ctx, ChunkBuf& cb, size_t in_bytes, size_t out3, size_t out1) {
@@ -703,6 +713,20 @@ void release_fft_plan(rtx_ctx* ctx) {
 constexpr size_t SMALL_PATH_BYTES = 4u << 20;
 constexpr size_t ZERO_COPY_BYTES = 16u << 10;  // rays + results of a zero-copy small trace
 
+// grow the pinned bounce buffer of the small paths (and its device twin) to `need` bytes
+int ensure_small(rtx_ctx* ctx, size_t need) {
+    if (need <= ctx->small_bytes) return 0;
+    if (ctx->small_host) CK(cudaFreeHost(ctx->small_host));
+    if (ctx->small_dev) CK(cudaFree(ctx->small_dev));
+    ctx->small_host = ctx->small_dev = nullptr;
+    ctx->small_bytes = 0;
+    const size_t nb = need < (256u << 10) ? (256u << 10) : need;
+    CK(cudaMallocHost(&ctx->small_host, nb));
+    CK(cudaMalloc(&ctx->small_dev, nb));
+    ctx->small_bytes = nb;
+    return 0;
+}
+
 // Latency path for small bundles (aim_chief / aim_marginal issue hundreds of
 // 1-3 ray traces, rayopt/system.py:507-555): one pinned bounce buffer, ONE
 // H2D of [y0|u0], the kernel with ld = N (per-thread stores, reference
@@ -714,16 +738,8 @@ int trace_host_small(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
                      size_t out_bytes) {
     const int rows = keep == RTX_KEEP_LAST ? 1 : S;
     const size_t need = in_bytes + out_bytes;
-    if (need > ctx->small_bytes) {
-        if (ctx->small_host) CK(cudaFreeHost(ctx->small_host));
-        if (ctx->small_dev) CK(cudaFree(ctx->small_dev));
-        ctx->small_host = ctx->small_dev = nullptr;
-        ctx->small_bytes = 0;
-        size_t nb = need < (256u << 10) ? (256u << 10) : need;
-        CK(cudaMallocHost(&ctx->small_host, nb));
-        CK(cudaMalloc(&ctx->small_dev, nb));
-        ctx->small_bytes = nb;
-    }
+    int rc = ensure_small(ctx, need);
+    if (rc) return rc;
     char* h = (char*)ctx->small_host;
     const size_t v3 = (size_t)N * 3 * sizeof(T), r3 = (size_t)rows * v3, r1 = r3 / 3;
     memcpy(h, y0, v3);
@@ -738,9 +754,10 @@ int trace_host_small(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
     if (!zero_copy) CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
     char* dY = d + in_bytes;
     char *dU = dY + r3, *dI = dU + r3, *dT = dI + r3;
-    int rc = trace_device<T>(ctx, surf, S, rot0, N, d, d + v3, clip, keep, N, Y ? dY : nullptr,
-                             U ? dU : nullptr, I ? dI : nullptr, Tt ? dT : nullptr,
-                             flags | RTX_STORE_DIRECT, ctx->stream, nullptr);
+    Launch<T> L(surf, S, rot0, clip, keep, N, flags | RTX_STORE_DIRECT);
+    rc = add_bundle<T>(ctx, L, surf, N, d, d + v3, Y ? dY : nullptr, U ? dU : nullptr,
+                       I ? dI : nullptr, Tt ? dT : nullptr);
+    if (!rc) rc = launch_trace<T>(ctx, L, ctx->stream);
     if (rc) return rc;
     if (!zero_copy)
         CK(cudaMemcpyAsync(h + in_bytes, dY, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -812,9 +829,10 @@ int trace_host(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
         }
         ctx->chunk_events.emplace_back(e0, e1);  // owned by ctx from here on
         CK(cudaEventRecord(e0, cb.stream));
-        rc = trace_device<T>(ctx, surf, S, rot0, n, cb.y0, cb.u0, clip, keep, C, Y ? cb.Y : nullptr,
-                             U ? cb.U : nullptr, I ? cb.I : nullptr, Tt ? cb.T : nullptr, flags,
-                             cb.stream, table);
+        Launch<T> L(surf, S, rot0, clip, keep, C, flags);
+        L.add(table, n, cb.y0, cb.u0, Y ? cb.Y : nullptr, U ? cb.U : nullptr, I ? cb.I : nullptr,
+              Tt ? cb.T : nullptr);
+        rc = launch_trace<T>(ctx, L, cb.stream);
         if (rc) {
             for (int b = 0; b < 2; ++b) cudaStreamSynchronize(ctx->chunk[b].stream);
             return rc;
@@ -914,33 +932,34 @@ int rtx_init(int device, rtx_ctx** out) {
         rtx_free(ctx);
         return rc;
     }
-    // tuning knobs (experiments; they override the per-call choice above)
+    // tuning knobs (experiments; they override choose_trace_cfg's choice)
+    Tuning& tu = ctx->tuning;
     if (const char* e = getenv("RTX_RPT")) {
         int v = atoi(e);
-        if (v == 1 || v == 2 || v == 4) ctx->default_rpt = v;
-        ctx->tuned = true;
+        if (v == 1 || v == 2 || v == 4) tu.rpt = v;
+        tu.tuned = true;
     }
     if (const char* e = getenv("RTX_WARPS")) {
         int v = atoi(e);
-        if (v == 8 || v == 16 || v == 32) ctx->warps = v;
+        if (v == 8 || v == 16 || v == 32) tu.warps = v;
     }
     if (const char* e = getenv("RTX_STORE")) {
         int v = atoi(e);
-        if (v == 1 || v == 2) ctx->store = v;
+        if (v == 1 || v == 2) tu.store = v;
     }
     if (const char* e = getenv("RTX_NBUF")) {
         int v = atoi(e);
-        if (v == 1 || v == 2) ctx->nbuf = v;
+        if (v == 1 || v == 2) tu.nbuf = v;
     }
     if (const char* e = getenv("RTX_CLUSTER")) {
         int v = atoi(e);
-        if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) ctx->cluster = v;
+        if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) tu.cluster = v;
     }
     if (getenv("RTX_WARPS") || getenv("RTX_STORE") || getenv("RTX_NBUF") || getenv("RTX_CLUSTER"))
-        ctx->tuned = true;
-    if (const char* e = getenv("RTX_LOCK")) ctx->lockstep = atoi(e) != 0;
-    if (const char* e = getenv("RTX_MAX_CTAS")) ctx->max_ctas_per_sm = atoi(e);
-    if (const char* e = getenv("RTX_TUNE")) ctx->tune = atoi(e);
+        tu.tuned = true;
+    if (const char* e = getenv("RTX_LOCK")) tu.lockstep = atoi(e) != 0;
+    if (const char* e = getenv("RTX_MAX_CTAS")) tu.max_ctas_per_sm = atoi(e);
+    if (const char* e = getenv("RTX_TUNE")) tu.tune = atoi(e);
     *out = ctx;
     return 0;
 }
@@ -1153,17 +1172,17 @@ int rtx_trace(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, 
     int rc = check_table(surf, S);
     if (rc) return rc;
     if (N < 0 || ld < N || !y0 || !u0) return RTX_E_BADARG;
-    if (keep != RTX_KEEP_ALL && keep != RTX_KEEP_LAST) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
     if (N == 0) return 0;
     CK(cudaSetDevice(ctx->device));
     CK(cudaEventRecord(ctx->k0, ctx->stream));
-    if (dtype == RTX_F64)
-        rc = trace_device<double>(ctx, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I, T, flags,
-                                  ctx->stream, nullptr);
-    else
-        rc = trace_device<float>(ctx, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I, T, flags,
-                                 ctx->stream, nullptr);
+    if (dtype == RTX_F64) {
+        Launch<double> L(surf, S, rot0, clip, keep, ld, flags);
+        rc = trace_registered(ctx, L, surf, N, y0, u0, Y, U, I, T);
+    } else {
+        Launch<float> L(surf, S, rot0, clip, keep, ld, flags);
+        rc = trace_registered(ctx, L, surf, N, y0, u0, Y, U, I, T);
+    }
     if (rc) return rc;
     CK(cudaEventRecord(ctx->k1, ctx->stream));
     ctx->kernel_timed = true;
@@ -1178,33 +1197,13 @@ int trace_batch(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S, con
                 const int64_t* N, const void* const* y0, const void* const* u0, int clip, int keep,
                 long long ld, void* const* Y, void* const* U, void* const* I, void* const* Tt,
                 unsigned flags) {
-    Batch<T> bt;
-    const void* tabs[RTX_MAX_BATCH];
-    long long nmax = 0;
+    Launch<T> L(surf[0], S, rot0, clip, keep, ld, flags);
     for (int b = 0; b < nb; ++b) {
-        const DevSurf<T>* tab = nullptr;
-        int rc = upload_table<T>(ctx, surf[b], S, ctx->stream, &tab, tabs, bt.n);
+        int rc = add_bundle<T>(ctx, L, surf[b], N[b], y0[b], u0[b], Y ? Y[b] : nullptr,
+                               U ? U[b] : nullptr, I ? I[b] : nullptr, Tt ? Tt[b] : nullptr);
         if (rc) return rc;
-        tabs[bt.n] = tab;
-        BatchItem<T>& it = bt.item[bt.n++];
-        it.table = tab;
-        it.y0 = (const T*)y0[b];
-        it.u0 = (const T*)u0[b];
-        it.Y = Y ? (T*)Y[b] : nullptr;
-        it.U = U ? (T*)U[b] : nullptr;
-        it.I = I ? (T*)I[b] : nullptr;
-        it.Tt = Tt ? (T*)Tt[b] : nullptr;
-        it.N = N[b];
-        it.tile0 = 0;
-        if (N[b] > nmax) nmax = N[b];
-        // every bundle must satisfy the alignment the bulk-store path needs
-        for (void* q : {(void*)it.Y, (void*)it.U, (void*)it.I, (void*)it.Tt})
-            if (reinterpret_cast<uintptr_t>(q) & 15u) flags |= RTX_STORE_DIRECT;
     }
-    // kernel configuration from the first bundle (same lens), N of the largest
-    return trace_device<T>(ctx, surf[0], S, rot0, nmax, y0[0], u0[0], clip, keep, ld,
-                           Y ? Y[0] : nullptr, U ? U[0] : nullptr, I ? I[0] : nullptr,
-                           Tt ? Tt[0] : nullptr, flags, ctx->stream, bt.item[0].table, nullptr, &bt);
+    return launch_trace<T>(ctx, L, ctx->stream);
 }
 }  // namespace
 
@@ -1215,26 +1214,19 @@ int rtx_trace_batch(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S,
                     const void* const* u0, int clip, int keep, int64_t ld, void* const* Y,
                     void* const* U, void* const* I, void* const* T, unsigned flags) {
     if (!ctx || nb < 1 || nb > RTX_MAX_BATCH || !surf || !N || !y0 || !u0) return RTX_E_BADARG;
-    if (keep != RTX_KEEP_ALL && keep != RTX_KEEP_LAST) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
     for (int b = 0; b < nb; ++b) {
         int rc = check_table(surf[b], S);
         if (rc) return rc;
         if (N[b] < 1 || ld < N[b] || !y0[b] || !u0[b]) return RTX_E_BADARG;
     }
     CK(cudaSetDevice(ctx->device));
-    unsigned* saved_mask = ctx->mask;  // per-ray side outputs are single-bundle features
-    void* saved_tsum = ctx->tsum;
-    ctx->mask = nullptr;
-    ctx->tsum = nullptr;
     CK(cudaEventRecord(ctx->k0, ctx->stream));
     int rc = dtype == RTX_F64
                  ? trace_batch<double>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I,
                                        T, flags)
                  : trace_batch<float>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I, T,
                                       flags);
-    ctx->mask = saved_mask;
-    ctx->tsum = saved_tsum;
     if (rc) return rc;
     CK(cudaEventRecord(ctx->k1, ctx->stream));
     ctx->kernel_timed = true;
@@ -1252,11 +1244,8 @@ int trace_batch_host(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S
                      const void* const* u0, int clip, int keep, void* const* Y, void* const* U,
                      void* const* I, void* const* Tt, unsigned flags) {
     const int rows = keep == RTX_KEEP_LAST ? 1 : S;
-    long long nmax = 0, nsum = 0;
-    for (int b = 0; b < nb; ++b) {
-        nmax = N[b] > nmax ? N[b] : nmax;
-        nsum += N[b];
-    }
+    long long nmax = 0;
+    for (int b = 0; b < nb; ++b) nmax = N[b] > nmax ? N[b] : nmax;
     const long long ld = (nmax + 31) / 32 * 32;  // one pitch for all bundles: whole 32-ray groups
     std::vector<size_t> in_off((size_t)nb);
     size_t o = 0;
@@ -1264,7 +1253,6 @@ int trace_batch_host(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S
         in_off[(size_t)b] = o;
         o += ((size_t)N[b] * 6 * sizeof(T) + 15) & ~size_t(15);
     }
-    (void)nsum;
     const size_t per3 = (size_t)rows * ld * 3 * sizeof(T), per1 = (size_t)rows * ld * sizeof(T);
     const size_t per_bundle = (Y ? per3 : 0) + (U ? per3 : 0) + (I ? per3 : 0) + (Tt ? per1 : 0);
     const size_t in_pad = (o + 255) & ~size_t(255);
@@ -1279,16 +1267,7 @@ int trace_batch_host(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S
         }
         return 0;
     }
-    if (need > ctx->small_bytes) {
-        if (ctx->small_host) CK(cudaFreeHost(ctx->small_host));
-        if (ctx->small_dev) CK(cudaFree(ctx->small_dev));
-        ctx->small_host = ctx->small_dev = nullptr;
-        ctx->small_bytes = 0;
-        const size_t cap = need < (256u << 10) ? (256u << 10) : need;
-        CK(cudaMallocHost(&ctx->small_host, cap));
-        CK(cudaMalloc(&ctx->small_dev, cap));
-        ctx->small_bytes = cap;
-    }
+    if (int rc = ensure_small(ctx, need)) return rc;
     char* h = (char*)ctx->small_host;
     char* d = (char*)ctx->small_dev;
     for (int b = 0; b < nb; ++b) {
@@ -1356,26 +1335,17 @@ int rtx_trace_batch_host(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, i
                          const void* const* u0, int clip, int keep, void* const* Y,
                          void* const* U, void* const* I, void* const* T, unsigned flags) {
     if (!ctx || nb < 1 || !surf || !N || !y0 || !u0) return RTX_E_BADARG;
-    if (keep != RTX_KEEP_ALL && keep != RTX_KEEP_LAST) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
     for (int b = 0; b < nb; ++b) {
         int rc = check_table(surf[b], S);
         if (rc) return rc;
         if (N[b] < 0 || (N[b] > 0 && (!y0[b] || !u0[b]))) return RTX_E_BADARG;
     }
     CK(cudaSetDevice(ctx->device));
-    unsigned* saved_mask = ctx->mask;
-    void* saved_tsum = ctx->tsum;
-    ctx->mask = nullptr;
-    ctx->tsum = nullptr;
-    int rc = dtype == RTX_F64
-                 ? trace_batch_host<double>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I,
-                                            T, flags)
-                 : trace_batch_host<float>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I,
-                                           T, flags);
-    ctx->mask = saved_mask;
-    ctx->tsum = saved_tsum;
-    return rc;
+    return dtype == RTX_F64 ? trace_batch_host<double>(ctx, nb, surf, S, rot0, N, y0, u0, clip,
+                                                       keep, Y, U, I, T, flags)
+                            : trace_batch_host<float>(ctx, nb, surf, S, rot0, N, y0, u0, clip,
+                                                      keep, Y, U, I, T, flags);
 }
 
 int rtx_trace_host(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, int dtype,
@@ -1385,21 +1355,12 @@ int rtx_trace_host(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* r
     int rc = check_table(surf, S);
     if (rc) return rc;
     if (N < 0 || !y0 || !u0) return RTX_E_BADARG;
-    if (keep != RTX_KEEP_ALL && keep != RTX_KEEP_LAST) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
     if (N == 0) return 0;
     CK(cudaSetDevice(ctx->device));
-    unsigned* saved = ctx->mask;  // mask / path sum belong to device-buffer traces
-    void* saved_tsum = ctx->tsum;
-    ctx->mask = nullptr;
-    ctx->tsum = nullptr;
     if (dtype == RTX_F64)
-        rc = trace_host<double>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
-    else
-        rc = trace_host<float>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
-    ctx->mask = saved;
-    ctx->tsum = saved_tsum;
-    return rc;
+        return trace_host<double>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
+    return trace_host<float>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
 }
 
 int rtx_set_mask_output(rtx_ctx* ctx, uint32_t* dmask) {
@@ -1447,7 +1408,7 @@ int rtx_trace_gather(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
     if (rc) return rc;
     if (N < 0 || !y0 || !u0 || npeers < 1 || npeers > 8 || !dst || dst_offset < 0)
         return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    if (!valid_keep_dtype(RTX_KEEP_LAST, dtype)) return RTX_E_BADARG;
     if (N == 0) return 0;
     PeerDst pd;
     pd.n = npeers;
@@ -1462,12 +1423,15 @@ int rtx_trace_gather(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
     CK(cudaSetDevice(ctx->device));
     CK(cudaEventRecord(ctx->k0, ctx->stream));
     const long long ld = ((N + 127) / 128) * 128;  // only the gather destinations are written
-    if (dtype == RTX_F64)
-        rc = trace_device<double>(ctx, surf, S, rot0, N, y0, u0, clip, RTX_KEEP_LAST, ld, nullptr,
-                                  nullptr, nullptr, nullptr, flags, ctx->stream, nullptr, &pd);
-    else
-        rc = trace_device<float>(ctx, surf, S, rot0, N, y0, u0, clip, RTX_KEEP_LAST, ld, nullptr,
-                                 nullptr, nullptr, nullptr, flags, ctx->stream, nullptr, &pd);
+    if (dtype == RTX_F64) {
+        Launch<double> L(surf, S, rot0, clip, RTX_KEEP_LAST, ld, flags);
+        L.peers = &pd;
+        rc = trace_registered(ctx, L, surf, N, y0, u0, nullptr, nullptr, nullptr, nullptr);
+    } else {
+        Launch<float> L(surf, S, rot0, clip, RTX_KEEP_LAST, ld, flags);
+        L.peers = &pd;
+        rc = trace_registered(ctx, L, surf, N, y0, u0, nullptr, nullptr, nullptr, nullptr);
+    }
     if (rc) return rc;
     CK(cudaEventRecord(ctx->k1, ctx->stream));
     ctx->kernel_timed = true;

@@ -36,7 +36,7 @@ DIRECT, WARP, CTA = 0, 1, 2                     # store paths (rtx_last_launch_c
 R1W8 = (1, WARP, 8, 2, 1)
 PER_RAY = (1, DIRECT, 8, 1, 1)
 MODES = {"exact": (np.float64, True), "fast": (np.float64, False), "fp32": (np.float32, False)}
-# the instantiated tuning space (rtx.cu launch_cfg), forced through RTX_* in a fresh engine
+# the instantiated tuning space (rtx.cu KERNELS), forced through RTX_* in a fresh engine
 FORCED = {
     "r1w8": (R1W8, 1), "r2w8": ((2, WARP, 8, 2, 1), 1), "r2c16": ((2, CTA, 16, 1, 1), 1),
     "r1c16": ((1, CTA, 16, 1, 1), 1), "r2c32": ((2, CTA, 32, 1, 1), 1),
@@ -440,7 +440,7 @@ def test_forced_configuration(sysdb, canon, forced, name, mode, cfg):
 
 # ---- the library's own choice on each side of every size threshold ---------
 def _by_size(dtype, newton, N):
-    """the default configuration of an untuned engine (rtx.cu trace_device) for
+    """the default configuration of an untuned engine (rtx.cu choose_trace_cfg) for
     aligned outputs with a pitch that is a multiple of 128"""
     if N <= 150_000:
         return R1W8
@@ -582,6 +582,8 @@ BATCHES = {
     "last_fp32": ("double_gauss", "fp32", [200_003, 145_679, 40_001], True,
                   (4, WARP, 16, 1, 1)),
     "small": ("cooke_asph", "fast", [60_001, 33_333, 77], False, R1W8),
+    # a single bundle is eligible for the clustered kernel
+    "one_bundle_cluster": ("double_gauss", "fast", [1_500_032], False, (2, CTA, 16, 1, 16)),
 }
 
 
@@ -643,6 +645,8 @@ GATHERS = {
     "fp32_newton": ("cooke_asph", "fp32", 200_000, 64, (2, WARP, 8, 2, 1)),
     "ragged": ("cooke_asph", "fast", 200_001, 64, PER_RAY),
     "small": ("rand_asph2", "fast", 40_000, 0, R1W8),
+    # the size takes the clustered kernel's configuration; a gather keeps it unclustered
+    "fp64_cluster_size": ("double_gauss", "fast", 1_500_032, 64, (2, CTA, 16, 1, 1)),
 }
 
 
