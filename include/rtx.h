@@ -569,6 +569,35 @@ int rtx_psf_bytes(rtx_ctx *ctx, int n, int pad, size_t *bytes);
 int rtx_psf(rtx_ctx *ctx, int dtype, int n, const void *o, int pad, void *psf,
             double *stats);
 
+/*
+ * Encircled-energy bins and line sums of a PSF -- what Analysis.opds
+ * (rayopt/analysis.py:330-346) reduces it to -- in one read of the PSF.
+ * psf is a DEVICE (nx, ny) array in the FFT order rtx_psf writes (RTX_F64
+ * only; RTX_F32 returns RTX_E_UNSUPPORTED).  The shifted index I (of
+ * np.fft.fftshift(psf)) is stored row (I - nx/2) mod nx, J likewise.  Host
+ * outputs, each may be NULL (then skipped):
+ *   ee (nbins,)  sum of the pixels whose bin about the centre (c0, c1), given
+ *                in the shifted frame, is b = trunc(sqrt((J-c1)^2 + (I-c0)^2))
+ *                with each operation rounded separately as numpy does:
+ *                polar_sum(fftshift(psf), (c0, c1), "azimuthal")
+ *                (special_sums.py:240-263, aspect 1, binsize 1),
+ *   lsf0 (ny,)   column sums sum_I psf[I, J],
+ *   lsf1 (nx,)   row sums sum_J psf[I, J], both in the stored order
+ *                (ifftshift(fftshift(psf).sum(i))).
+ * nbins must be np.bincount's length, 1 + the largest bin, which lies at a
+ * corner of the array.  Every sum is taken in a fixed order (the same PSF and
+ * centre give the same bits); the pixels are >= 0, so each sum's relative
+ * error is at most (L + 200) DBL_EPSILON/2, L = ceil(tiles/132) with
+ * tiles = ceil(nx/64) ceil(ny/64).  RTX_E_BADARG for NULL ctx or psf, nx or ny < 1, a non-finite
+ * centre, another nbins, or a negative or non-finite pixel (found by the
+ * kernel; outputs then unspecified).  Scratch of 133 (nbins + nx + ny) doubles
+ * is kept in the context; RTX_E_NOMEM before allocating when it does not fit.
+ * Synchronous; rtx_last_kernel_ms gives the device time of the call.
+ */
+int rtx_psf_profiles(rtx_ctx *ctx, int dtype, int64_t nx, int64_t ny,
+                     const void *psf, double c0, double c1, int64_t nbins,
+                     double *ee, double *lsf0, double *lsf1);
+
 #ifdef __cplusplus
 }
 #endif

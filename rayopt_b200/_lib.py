@@ -74,6 +74,8 @@ SYMBOLS = {
     "rtx_grid_linear": (_i, [_vp, _i, _i64, _vp, _vp, _i64, _vp, _vp, _i, _vp, _vp, _vp]),
     "rtx_psf_bytes": (_i, [_vp, _i, _i, C.POINTER(_sz)]),
     "rtx_psf": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
+    "rtx_psf_profiles": (_i, [_vp, _i, _i64, _i64, _vp, C.c_double, C.c_double, _i64,
+                              _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -12,6 +12,7 @@
 #include <sys/syscall.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <cctype>
 #include <cmath>
 #include <cstdio>
@@ -112,6 +113,9 @@ struct rtx_ctx {
     void* fft_work = nullptr;
     size_t fft_work_bytes = 0;
     double* d_psf_red = nullptr;  // partial sums, the finite count and the stats
+    // rtx_psf_profiles: per-block partial rows, their sum and the pixel flag
+    double* d_prof = nullptr;
+    size_t prof_cap = 0;
 };
 
 namespace {
@@ -982,6 +986,7 @@ int rtx_free(rtx_ctx* ctx) {
     if (ctx->d_winner) cudaFree(ctx->d_winner);
     release_fft_plan(ctx);
     if (ctx->d_psf_red) cudaFree(ctx->d_psf_red);
+    if (ctx->d_prof) cudaFree(ctx->d_prof);
     if (ctx->small_host) cudaFreeHost(ctx->small_host);
     if (ctx->small_dev) cudaFree(ctx->small_dev);
     if (ctx->t0) cudaEventDestroy(ctx->t0);
@@ -2041,6 +2046,70 @@ int rtx_psf(rtx_ctx* ctx, int dtype, int n, const void* o, int pad, void* psf, d
     if (stats)
         CK(cudaMemcpyAsync(stats, d_stats, 5 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+int rtx_psf_profiles(rtx_ctx* ctx, int dtype, int64_t nx, int64_t ny, const void* psf, double c0,
+                     double c1, int64_t nbins, double* ee, double* lsf0, double* lsf1) {
+    if (!ctx || !psf || nx < 1 || ny < 1 || !std::isfinite(c0) || !std::isfinite(c1))
+        return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64) return RTX_E_BADARG;
+    if (nx > INT64_MAX / 8 / ny) return RTX_E_BADARG;
+    // np.bincount's length: 1 + the largest bin, which sits at a corner
+    long long last = 0;
+    for (long long I : {0ll, (long long)nx - 1})
+        for (long long J : {0ll, (long long)ny - 1}) {
+            volatile double i = (double)I - c0, j = (double)J - c1;
+            volatile double s = j * j + i * i;
+            if (!(s < 0x1p100)) return RTX_E_NOMEM;  // radius >= 2^50: no such histogram fits
+            last = std::max(last, profile_bin((double)I, (double)J, c0, c1));
+        }
+    if (nbins != last + 1) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    const long long stride = nbins + nx + ny;
+    // PROF_BLOCKS partial rows, their sum, the flag
+    const size_t need = ((size_t)(PROF_BLOCKS + 1) * stride + 1) * sizeof(double);
+    if (need > ctx->prof_cap) {
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        if (need > free_b + ctx->prof_cap) return RTX_E_NOMEM;  // nothing allocated
+        if (ctx->d_prof) CK(cudaFree(ctx->d_prof));
+        ctx->d_prof = nullptr;
+        ctx->prof_cap = 0;
+        if (cudaMalloc((void**)&ctx->d_prof, need) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->d_prof = nullptr;
+            return RTX_E_NOMEM;
+        }
+        ctx->prof_cap = need;
+    }
+    double* part = ctx->d_prof;
+    double* out = part + (long long)PROF_BLOCKS * stride;
+    int* flag = reinterpret_cast<int*>(out + stride);
+    long long grid = (stride + 255) / 256;
+    const long long cap = (long long)ctx->sm_count * 8;
+    if (grid > cap) grid = cap;
+    CK(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+    CK(cudaEventRecord(ctx->k0, ctx->stream));
+    profile_tiles_kernel<<<PROF_BLOCKS, PROF_WARPS * 32, 0, ctx->stream>>>(
+        (const double*)psf, nx, ny, c0, c1, nbins, part, stride, flag);
+    profile_combine_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(part, PROF_BLOCKS, stride, out);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, ctx->stream));
+    ctx->kernel_timed = true;
+    int h_flag = 0;
+    CK(cudaMemcpyAsync(&h_flag, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (ee) CK(cudaMemcpyAsync(ee, out, nbins * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    if (lsf1)
+        CK(cudaMemcpyAsync(lsf1, out + nbins, nx * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    if (lsf0)
+        CK(cudaMemcpyAsync(lsf0, out + nbins + nx, ny * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (h_flag & 1) return RTX_E_BADARG;        // a negative or non-finite pixel
+    if (h_flag) return RTX_E_UNSUPPORTED;       // a tile over PROF_TILE_BINS bins: not reached below 2^50
     return 0;
 }
 

@@ -233,4 +233,170 @@ __global__ void psf_stats_kernel(const double* __restrict__ part, int nblocks,
     for (int q = 0; q < 4; ++q) stats[1 + q] = r[q];
 }
 
+// ---- radial and line sums of a PSF (Analysis.opds, rayopt/analysis.py:330-346)
+//
+// The PSF is read in its stored FFT order; (I, J) are the indices of the
+// fftshifted image, stored at ((I - nx/2) mod nx, (J - ny/2) mod ny).  Bin of
+// (I, J) about the centre (c0, c1): trunc(sqrt((J - c1)^2 + (I - c0)^2)) with
+// numpy's separately rounded operations (polar_sum, aspect 1, binsize 1).
+//
+// Deterministic without float atomics: PROF_BLOCKS blocks (a constant, not the
+// SM count) each take a fixed contiguous range of 64 x 64 tiles of the shifted
+// image and accumulate into block-private rows of partial sums (bins, row sums,
+// column sums) in tile order; profile_combine_kernel then sums the rows in
+// block order.  Inside a tile each warp owns 4 rows: along a row the bin is
+// monotone on each side of the centre column, so equal (bin, side) keys are
+// contiguous lanes and a segmented scan sums them in a fixed order; the
+// segment tails add into the warp's shared histogram (side j < 0 first), and
+// the 16 warp histograms are summed in warp order at the end of the tile.
+constexpr int PROF_TILE = 64;
+constexpr int PROF_WARPS = 16;                     // 512 threads, 4 rows each
+constexpr int PROF_ROWS = PROF_TILE / PROF_WARPS;
+constexpr int PROF_TILE_BINS = 96;                 // a 64 x 64 tile spans <= 91 bins
+constexpr int PROF_BLOCKS = 132;
+
+__host__ __device__ __forceinline__ long long profile_bin(double I, double J, double c0, double c1) {
+#ifdef __CUDA_ARCH__
+    const double i = __dsub_rn(I, c0), j = __dsub_rn(J, c1);
+    return (long long)__dsqrt_rn(__dadd_rn(__dmul_rn(j, j), __dmul_rn(i, i)));
+#else
+    volatile double i = I - c0, j = J - c1;  // volatile: no contraction on the host
+    volatile double jj = j * j, ii = i * i;
+    volatile double s = jj + ii;
+    return (long long)sqrt((double)s);
+#endif
+}
+
+// stored index of the shifted index k along an axis of m
+__device__ __forceinline__ long long unshift(long long k, long long m) {
+    const long long s = k - m / 2;
+    return s < 0 ? s + m : s;
+}
+
+// partial rows: block g owns part[g*stride, (g+1)*stride) = [bins | row sums (nx) |
+// column sums (ny)], the rows and columns in stored order.  flag bit 0: a
+// negative or non-finite pixel; bit 1: a tile spanned more than PROF_TILE_BINS
+// bins (cannot happen for in-range centres; reported rather than dropped)
+__global__ void __launch_bounds__(PROF_WARPS * 32) profile_tiles_kernel(
+    const double* __restrict__ psf, long long nx, long long ny, double c0, double c1,
+    long long nbins, double* __restrict__ part, long long stride, int* __restrict__ flag) {
+    __shared__ double hist[PROF_WARPS][PROF_TILE_BINS];
+    __shared__ double cols[PROF_WARPS][PROF_TILE];
+    __shared__ long long s_b0;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    double* mine = part + (long long)blockIdx.x * stride;
+    double* rows = mine + nbins;
+    double* colsum = rows + nx;
+    for (long long k = threadIdx.x; k < stride; k += blockDim.x) mine[k] = 0.0;
+    for (int k = threadIdx.x; k < PROF_WARPS * PROF_TILE_BINS; k += blockDim.x)
+        (&hist[0][0])[k] = 0.0;
+    const long long ntr = (nx + PROF_TILE - 1) / PROF_TILE, ntc = (ny + PROF_TILE - 1) / PROF_TILE;
+    const long long T = ntr * ntc;
+    const long long t0 = T * blockIdx.x / gridDim.x, t1 = T * (blockIdx.x + 1) / gridDim.x;
+    int bad = 0;
+    for (long long t = t0; t < t1; ++t) {
+        const long long I0 = (t / ntc) * PROF_TILE, J0 = (t % ntc) * PROF_TILE;
+        const long long I1 = min(I0 + PROF_TILE, nx) - 1, J1 = min(J0 + PROF_TILE, ny) - 1;
+        if (threadIdx.x == 0) {
+            // the lowest bin of the tile: the radius is monotone in |I - c0| and
+            // |J - c1|, whose minima over the tile's integers are at a clamped
+            // floor or ceil of the centre
+            long long b0 = LLONG_MAX;
+            const double fi = floor(c0), fj = floor(c1);
+            for (int a = 0; a < 2; ++a)
+                for (int b = 0; b < 2; ++b) {
+                    const double I = fmin(fmax(fi + a, (double)I0), (double)I1);
+                    const double J = fmin(fmax(fj + b, (double)J0), (double)J1);
+                    b0 = min(b0, profile_bin(I, J, c0, c1));
+                }
+            s_b0 = b0;
+        }
+        __syncthreads();
+        const long long b0 = s_b0;
+        // loads first: 8 pixels per lane in flight
+        double v[PROF_ROWS][2];
+        bool ok[PROF_ROWS][2];
+#pragma unroll
+        for (int r = 0; r < PROF_ROWS; ++r) {
+            const long long I = I0 + w * PROF_ROWS + r;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const long long J = J0 + 32 * h + lane;
+                ok[r][h] = I <= I1 && J <= J1;
+                v[r][h] = ok[r][h] ? __ldcs(psf + unshift(I, nx) * ny + unshift(J, ny)) : 0.0;
+            }
+        }
+        double csum[2] = {0.0, 0.0};
+#pragma unroll
+        for (int r = 0; r < PROF_ROWS; ++r) {
+            const long long I = I0 + w * PROF_ROWS + r;
+            double rsum = 0.0;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const double x = v[r][h];
+                const long long J = J0 + 32 * h + lane;
+                if (ok[r][h] && !(x >= 0.0 && x <= DBL_MAX)) bad |= 1;
+                csum[h] = __dadd_rn(csum[h], x);
+                rsum = __dadd_rn(rsum, x);
+                long long key = -1;  // 2 bin + (j >= 0); -1 outside the array
+                if (ok[r][h]) {
+                    const long long b = profile_bin((double)I, (double)J, c0, c1) - b0;
+                    if (b < 0 || b >= PROF_TILE_BINS) bad |= 2;
+                    else key = 2 * b + (__dsub_rn((double)J, c1) >= 0.0 ? 1 : 0);
+                }
+                // segmented inclusive scan over runs of equal keys
+                const long long prev = __shfl_up_sync(0xffffffffu, key, 1);
+                const unsigned heads = __ballot_sync(0xffffffffu, lane == 0 || prev != key);
+                const int start = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
+                double s = x;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const double u = __shfl_up_sync(0xffffffffu, s, d);
+                    if (lane - d >= start) s = __dadd_rn(s, u);
+                }
+                const bool tail = lane == 31 || ((heads >> (lane + 1)) & 1u);
+                if (tail && key >= 0 && (key & 1) == 0) hist[w][key >> 1] += s;
+                __syncwarp();
+                if (tail && key >= 0 && (key & 1) == 1) hist[w][key >> 1] += s;
+                __syncwarp();
+            }
+            for (int off = 16; off; off >>= 1) rsum = __dadd_rn(rsum, __shfl_xor_sync(0xffffffffu, rsum, off));
+            if (lane == 0 && I <= I1) rows[unshift(I, nx)] += rsum;
+        }
+        cols[w][lane] = csum[0];
+        cols[w][lane + 32] = csum[1];
+        __syncthreads();
+        const int k = threadIdx.x;
+        if (k < PROF_TILE) {
+            if (J0 + k <= J1) {
+                double s = 0.0;
+                for (int q = 0; q < PROF_WARPS; ++q) s = __dadd_rn(s, cols[q][k]);
+                colsum[unshift(J0 + k, ny)] += s;
+            }
+        } else if (k < PROF_TILE + PROF_TILE_BINS) {
+            const int b = k - PROF_TILE;
+            double s = 0.0;
+            for (int q = 0; q < PROF_WARPS; ++q) {
+                s = __dadd_rn(s, hist[q][b]);
+                hist[q][b] = 0.0;
+            }
+            if (b0 + b < nbins) mine[b0 + b] += s;
+        }
+        __syncthreads();
+    }
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    if (lane == 0 && bad) atomicOr(flag, bad);
+}
+
+// out[k] = sum over the blocks' partial rows, in block order
+__global__ void __launch_bounds__(256) profile_combine_kernel(const double* __restrict__ part, int nblocks,
+                                                              long long stride, double* __restrict__ out) {
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < stride;
+         k += (long long)gridDim.x * blockDim.x) {
+        double s = 0.0;
+        for (int g = 0; g < nblocks; ++g) s = __dadd_rn(s, part[g * stride + k]);
+        out[k] = s;
+    }
+}
+
 }  // namespace rtx

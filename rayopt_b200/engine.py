@@ -781,6 +781,37 @@ class Engine:
         return dict(count=int(raw[0]), sum=float(raw[1]), max=float(raw[2]),
                     cp=float(raw[3]*step), cq=float(raw[4]*step))
 
+    @staticmethod
+    def profile_nbins(shape, center):
+        """np.bincount's length for the radial bins of an array of `shape`
+        about `center`: 1 + the largest bin, at a corner (polar_sum's
+        arithmetic, aspect 1, binsize 1); 0 for a non-finite centre or a
+        radius of 2^50 or more, which rtx_psf_profiles refuses"""
+        i = np.array([0., shape[0] - 1]) - float(center[0])
+        j = np.array([0., shape[1] - 1]) - float(center[1])
+        with np.errstate(all="ignore"):
+            r = np.sqrt(j[None, :]*j[None, :] + i[:, None]*i[:, None])
+        if not (r < 2.**50).all():
+            return 0
+        return int(r.astype(np.int64).max()) + 1
+
+    def psf_profiles(self, psf, center):
+        """rtx_psf_profiles of the PSF `psf` (DEVICE (nx, ny) FP64, the FFT
+        order of ``psf``) about `center` (c0, c1) in the fftshifted frame:
+        (ee_bins, lsf0, lsf1) as numpy arrays -- polar_sum(fftshift(psf),
+        center, "azimuthal") and the column and row sums in the stored order
+        (ifftshift(fftshift(psf).sum(i)) for i = 0, 1).  Raises RtxError for a
+        negative or non-finite pixel."""
+        if len(psf.shape) != 2 or psf.dtype != np.float64:
+            raise ValueError("psf must be a 2-d FP64 device array")
+        nx, ny = psf.shape
+        c0, c1 = float(center[0]), float(center[1])
+        nbins = self.profile_nbins(psf.shape, (c0, c1))
+        ee, lsf0, lsf1 = np.empty(nbins), np.empty(ny), np.empty(nx)
+        check(self.lib.rtx_psf_profiles(self.ctx, RTX_F64, nx, ny, psf.ptr, c0, c1, nbins,
+                                        ptr(ee), ptr(lsf0), ptr(lsf1)))
+        return ee, lsf0, lsf1
+
 
 _default = {}
 

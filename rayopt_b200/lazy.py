@@ -475,6 +475,37 @@ class ResidentMixin:
             return p, q, psf
         return p, q, out
 
+    def psf_profiles(self, pad=4, resample=4, **kwargs):
+        """The encircled energy and MTF Analysis.opds (rayopt/analysis.py:
+        319-346) takes from ``psf``, with the PSF kept in HBM: ``psf_device``
+        (download=False), its centroid (x0, y0) = (cp, cq) from the device
+        stats, dx from the fftshifted p axis after subtracting x0 as Analysis
+        does, and rtx_psf_profiles about (nx/2 + x0/dx, ny/2 + y0/dx) (true
+        division: for odd sizes half a pixel from the fftshift origin, as in
+        Analysis).  Returns a dict: stats, x0, y0, dx, center, xe (bin radii),
+        ee (cumulative), of (frequencies) and mtf (axis 0, axis 1); the 1-d
+        inverse FFTs of the line sums run on the host."""
+        p, q, out = self.psf_device(pad, resample, download=False, **kwargs)
+        try:
+            st = self.psf_stats
+            x0, y0 = st["cp"], st["cq"]
+            xs = np.fft.fftshift(p[:, 0])
+            dx = (xs[1] - x0) - (xs[0] - x0)
+            nx, ny = out.shape
+            center = (nx/2 + x0/dx, ny/2 + y0/dx)
+            bins, lsf0, lsf1 = self._engine().psf_profiles(out, center)
+        finally:
+            out.free()
+        size = nx*ny
+        mtf = []
+        for lsf in (lsf0, lsf1):
+            ot = np.fft.ifft(lsf*size**.5)
+            mtf.append(np.absolute(ot[:ot.size//2]))
+        of = np.fft.fftfreq(lsf0.size, dx)[:lsf0.size//2]
+        ee = np.cumsum(bins)
+        return dict(stats=st, x0=x0, y0=y0, dx=dx, center=center, xe=np.arange(ee.size)*dx,
+                    ee=ee, of=of, mtf=tuple(mtf))
+
 
 class ResidentTrace(ResidentMixin):
     """Standalone resident drop-in (no rayopt import needed) with launch rays

@@ -13,7 +13,13 @@ Delaunay triangulation with its barycentric transforms, rtx_grid_linear (uploads
 the kernel), rtx_psf (pupil, cuFFT, |.|^2, stats; CUDA events) and the
 download of the PSF.  Host path: griddata's evaluation on the SAME
 triangulation (LinearNDInterpolator) and the padded numpy fft2 + |.|^2.  The
-two PSFs are compared in the same run.  Every shape is warmed once; the
+two PSFs are compared in the same run.
+
+Encircled energy and MTF (Analysis.opds, rayopt/analysis.py:330-346) of the
+device's PSF about its centroid: on the device rtx_psf_profiles (the call, its
+kernels by CUDA events and the PSF bytes read over that time), on the host the
+fftshift, polar_sum, line sums and the two 1-d inverse FFTs of the downloaded
+PSF (whose download is the device path's download row).  Every shape is warmed once; the
 median and the range of --reps repetitions are printed (host path at 1e6 rays:
 one repetition).
 """
@@ -50,6 +56,7 @@ def main():
     import yaml
     from scipy.interpolate import LinearNDInterpolator
     from scipy.spatial import Delaunay
+    import profile_oracle
     import psf_oracle
     import ref_shim
     import systems_yaml
@@ -88,16 +95,44 @@ def main():
             out, raw = eng.psf(o, 4)
             t4 = time.perf_counter()
             st["psf_kernels_ms"] = eng.last_kernel_ms()
-            psf = out.download()
+            # encircled-energy bins and line sums about the centroid, as
+            # ResidentMixin.psf_profiles takes them
+            f = psf_oracle.frequencies(xs, 4*n, wl, radius)
+            ps = eng.psf_stats(raw, f)
+            cp, cq, fs = ps["cp"], ps["cq"], np.fft.fftshift(f)
+            dx = (fs[1] - cp) - (fs[0] - cp)
+            center = (2*n + cp/dx, 2*n + cq/dx)
             t5 = time.perf_counter()
+            prof = eng.psf_profiles(out, center)
+            t6 = time.perf_counter()
+            st["profiles_kernels_ms"] = ms = eng.last_kernel_ms()
+            st["profiles_read_GBps"] = out.nbytes/ms/1e6
+            psf = out.download()
+            t7 = time.perf_counter()
             o.free()
             out.free()
             st.update(opd_rays_s=t1 - t0, triangulation_s=t2 - t1, regrid_call_s=t3 - t2,
-                      psf_call_s=t4 - t3, download_s=t5 - t4, total_s=t5 - t0)
-            return st, (x, y, t, tri, xs, ys, n), psf
+                      psf_call_s=t4 - t3, profiles_call_s=t6 - t5, download_s=t7 - t6,
+                      total_s=t7 - t0 - (t6 - t5))
+            return st, (x, y, t, tri, xs, ys, n, center, prof), psf
+
+        def host_profiles(psf, center):
+            """Analysis.opds's reduction of the downloaded PSF"""
+            t0 = time.perf_counter()
+            s = np.fft.fftshift(psf)
+            t1 = time.perf_counter()
+            bins = profile_oracle.polar_sum_azimuthal(s, center)
+            t2 = time.perf_counter()
+            lsf = [np.fft.ifftshift(s.sum(i)) for i in range(2)]
+            t3 = time.perf_counter()
+            mtf = [np.absolute(np.fft.ifft(v*s.size**.5)) for v in lsf]
+            t4 = time.perf_counter()
+            return dict(prof_fftshift_s=t1 - t0, prof_polar_sum_s=t2 - t1,
+                        prof_line_sums_s=t3 - t2, prof_ifft_s=t4 - t3,
+                        prof_host_total_s=t4 - t0), (bins, *lsf)
 
         def host(data):
-            x, y, t, tri, xs, ys, n = data
+            x, y, t, tri, xs, ys, n = data[:7]
             t0 = time.perf_counter()
             o = LinearNDInterpolator(tri, t, fill_value=np.nan)(xs, ys)
             t1 = time.perf_counter()
@@ -112,8 +147,14 @@ def main():
         hst = [host(data) for _ in range(hreps)]
         psf_h = hst[-1][1]
         err = float(np.abs(psf_d - psf_h).max()/psf_h.max())
+        # the host's profile path on the device's PSF (its download is timed
+        # on the device side); one run at 1e6 rays
+        hprof = [host_profiles(psf_d, data[7]) for _ in range(hreps)]
+        perr = max(float(np.abs(np.cumsum(a) - np.cumsum(b)).max())
+                   for a, b in zip(data[8], hprof[-1][1]))
+        hst = [(dict(h[0], **hp[0]), h[1]) for h, hp in zip(hst, hprof)]
         row = dict(nrays=g.nrays, n=data[6], padded=4*data[6], rel_err_vs_host=err,
-                   host_reps=hreps, card=info)
+                   profiles_cumsum_err_vs_host=perr, host_reps=hreps, card=info)
         for key in dev[0][0]:
             v = [d[0][key] for d in dev]
             row[key] = (statistics.median(v), min(v), max(v))
