@@ -359,6 +359,14 @@ int rtx_selftest_math(rtx_ctx *ctx, int64_t n, const double *a, const double *b,
  */
 int rtx_selftest_math2(rtx_ctx *ctx, int64_t n, const double *a, const double *b,
                        const double *c, double *out);
+/*
+ * The exact predicates of rtx_delaunay: for n host point quadruples pts[8i..8i+7]
+ * = (a, b, c, d) writes 2*n ints to `out` (host): the sign of orient2d(a, b, c)
+ * (> 0: counter-clockwise) and of incircle(a, b, c, d) (> 0: d strictly inside
+ * the circle through a, b, c when they are counter-clockwise).  Exact for
+ * coordinates in rtx_delaunay's domain.
+ */
+int rtx_selftest_predicates(rtx_ctx *ctx, int64_t n, const double *pts, int *out);
 
 /* ---- fused last-surface reductions (geometric_trace.py:171-183) ------- */
 /*
@@ -597,6 +605,39 @@ int rtx_psf(rtx_ctx *ctx, int dtype, int n, const void *o, int pad, void *psf,
 int rtx_psf_profiles(rtx_ctx *ctx, int dtype, int64_t nx, int64_t ny,
                      const void *psf, double c0, double c1, int64_t nbins,
                      double *ee, double *lsf0, double *lsf1);
+
+/*
+ * Delaunay triangulation of M DEVICE points pts (M,2) on the device, in the
+ * layout scipy.spatial.Delaunay gives and rtx_grid_linear takes (RTX_F64 only;
+ * RTX_F32 returns RTX_E_UNSUPPORTED).  DEVICE outputs with room for 2*M
+ * triangles; *T (host) receives their number:
+ *   simplices (T,3) int32, counter-clockwise,
+ *   neighbors (T,3) int32 or NULL: the triangle opposite vertex k, -1 on the hull,
+ *   transform (T,3,2) FP64 or NULL: {Tinv, r}, r the last vertex and Tinv the
+ *     inverse (explicit 2x2 formula) of T = [v0 - r, v1 - r] as columns.
+ * The triangulation is exactly Delaunay: orient2d and incircle are exact
+ * (rtx_selftest_predicates), an edge is flipped only when its opposite vertex
+ * is strictly inside the circumcircle, and the triangles cover exactly the
+ * convex hull, collinear hull points included, with no zero-area triangle.
+ * Where the Delaunay triangulation is unique it is scipy's; among cocircular
+ * points the choice is deterministic but may differ from qhull's.  An exact
+ * duplicate of a point is not a vertex (the lowest index is kept).  The same
+ * points give the same bits in every call and context.
+ * Domain: every coordinate is 0 or 2^-200 <= |x| <= 2^200, so that no
+ * product of the exact predicates underflows or overflows.
+ * RTX_E_BADARG for M < 3 or M >= 2^30, a non-finite point or a coordinate
+ * outside the domain, and when all points are collinear (scipy raises
+ * QhullError).  The workspace (rtx_delaunay_bytes) is kept in the context;
+ * RTX_E_NOMEM before allocating anything when it does not fit in free device
+ * memory.  Not included there: the exact incircle's 3.3 KB stack frame, for
+ * which the driver reserves local memory on every resident thread at the
+ * first call in a context and keeps it (592 MB on an H100 80GB).  Synchronous; rtx_last_kernel_ms gives the device time of the call.
+ */
+int rtx_delaunay(rtx_ctx *ctx, int dtype, int64_t M, const void *pts, int64_t *T,
+                 int32_t *simplices, int32_t *neighbors, void *transform);
+/* device bytes of the workspace rtx_delaunay needs for M points (allocated by
+ * a call only when the context keeps a smaller one) */
+int rtx_delaunay_bytes(rtx_ctx *ctx, int64_t M, size_t *bytes);
 
 #ifdef __cplusplus
 }

@@ -76,6 +76,9 @@ SYMBOLS = {
     "rtx_psf": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "rtx_psf_profiles": (_i, [_vp, _i, _i64, _i64, _vp, C.c_double, C.c_double, _i64,
                               _vp, _vp, _vp]),
+    "rtx_selftest_predicates": (_i, [_vp, _i64, _vp, _vp]),
+    "rtx_delaunay": (_i, [_vp, _i, _i64, _vp, C.POINTER(_i64), _vp, _vp, _vp]),
+    "rtx_delaunay_bytes": (_i, [_vp, _i64, C.POINTER(_sz)]),
 }
 
 _lib = None

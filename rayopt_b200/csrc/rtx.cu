@@ -5,6 +5,7 @@
 #include "../../include/rtx.h"
 #include "rtx_device.cuh"
 #include "rtx_psf.cuh"
+#include "rtx_delaunay.cuh"
 
 #include <cufft.h>  // types only: the library is opened at run time (rtx_psf)
 #include <dlfcn.h>
@@ -116,6 +117,9 @@ struct rtx_ctx {
     // rtx_psf_profiles: per-block partial rows, their sum and the pixel flag
     double* d_prof = nullptr;
     size_t prof_cap = 0;
+    // rtx_delaunay: slots, adjacency and point-location workspace
+    void* d_dt = nullptr;
+    size_t dt_cap = 0;
 };
 
 namespace {
@@ -987,6 +991,7 @@ int rtx_free(rtx_ctx* ctx) {
     release_fft_plan(ctx);
     if (ctx->d_psf_red) cudaFree(ctx->d_psf_red);
     if (ctx->d_prof) cudaFree(ctx->d_prof);
+    if (ctx->d_dt) cudaFree(ctx->d_dt);
     if (ctx->small_host) cudaFreeHost(ctx->small_host);
     if (ctx->small_dev) cudaFree(ctx->small_dev);
     if (ctx->t0) cudaEventDestroy(ctx->t0);
@@ -2110,6 +2115,196 @@ int rtx_psf_profiles(rtx_ctx* ctx, int dtype, int64_t nx, int64_t ny, const void
     CK(cudaStreamSynchronize(ctx->stream));
     if (h_flag & 1) return RTX_E_BADARG;        // a negative or non-finite pixel
     if (h_flag) return RTX_E_UNSUPPORTED;       // a tile over PROF_TILE_BINS bins: not reached below 2^50
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- Delaunay triangulation of the exit pupil (rtx_delaunay.cuh) ----------
+namespace {
+
+constexpr long long DT_MAX_POINTS = (1ll << 30) - 1;  // 2M slots and the point index fit in int32
+
+// the workspace of M points (slots for 2M triangles) carved from `base`;
+// returns its size (base may be NULL to count only)
+size_t dt_carve(void* base, long long M, const void* pts, dt::Work* w) {
+    const long long S = 2 * M, nb = (S + dt::SCAN_THREADS - 1) / dt::SCAN_THREADS;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        void* p = base ? (char*)base + off : nullptr;
+        off += (bytes + 255) / 256 * 256;
+        return p;
+    };
+    dt::Work x{};
+    x.p = (const double2*)pts;
+    x.M = M;
+    x.pick = (unsigned long long*)take(S * 8);
+    x.vote = (unsigned long long*)take(S * 8);
+    x.ext = (int2*)take(S * 8);
+    x.tv = (int*)take(S * 12);
+    x.tn = (int*)take(S * 12);
+    x.mod = (int*)take(S * 4);
+    x.chk = (int*)take(S * 4);
+    x.op = (int*)take(S * 4);
+    x.flag = (int*)take(S * 4);
+    x.rank = (int*)take(S * 4);
+    x.bsum = (int*)take((nb + 1) * 4);
+    x.loc = (int*)take(M * 4);
+    x.cnt = (unsigned*)take(dt::C_N * 4);
+    x.lex = (long long*)take((2 * dt::LEX_BLOCKS + 2) * 8);
+    x.seed_key = (unsigned long long*)take(8);
+    if (w) *w = x;
+    return off;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rtx_delaunay_bytes(rtx_ctx* ctx, int64_t M, size_t* bytes) {
+    if (!ctx || !bytes || M < 3 || M > DT_MAX_POINTS) return RTX_E_BADARG;
+    *bytes = dt_carve(nullptr, M, nullptr, nullptr);
+    return 0;
+}
+
+int rtx_selftest_predicates(rtx_ctx* ctx, int64_t n, const double* pts, int* out) {
+    if (!ctx || n < 1 || !pts || !out) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    struct Bufs {  // freed on every return path
+        double* q = nullptr;
+        int* o = nullptr;
+        ~Bufs() {
+            cudaFree(q);
+            cudaFree(o);
+        }
+    } d;
+    CK(cudaMalloc((void**)&d.q, 8 * n * sizeof(double)));
+    CK(cudaMalloc((void**)&d.o, 2 * n * sizeof(int)));
+    CK(cudaMemcpyAsync(d.q, pts, 8 * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    dt::selftest_predicates_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.q, n, d.o);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, d.o, 2 * n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+int rtx_delaunay(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, int64_t* T, int32_t* simplices,
+                 int32_t* neighbors, void* transform) {
+    if (!ctx || !pts || !T || !simplices) return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64 || M < 3 || M > DT_MAX_POINTS) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    ctx->kernel_timed = false;  // until the call completes
+    const size_t need = dt_carve(nullptr, M, nullptr, nullptr);
+    if (need > ctx->dt_cap) {
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        if (need > free_b + ctx->dt_cap) return RTX_E_NOMEM;  // nothing allocated
+        if (ctx->d_dt) CK(cudaFree(ctx->d_dt));
+        ctx->d_dt = nullptr;
+        ctx->dt_cap = 0;
+        if (cudaMalloc(&ctx->d_dt, need) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->d_dt = nullptr;
+            return RTX_E_NOMEM;
+        }
+        ctx->dt_cap = need;
+    }
+    dt::Work w;
+    dt_carve(ctx->d_dt, M, pts, &w);
+    cudaStream_t st = ctx->stream;
+    auto grid = [&](long long items) {
+        long long b = (items + 255) / 256, cap = (long long)ctx->sm_count * 16;
+        return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
+    };
+    unsigned cnt[dt::C_N];
+    auto counters = [&]() -> int {  // launches so far checked, counters read back
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(cnt, w.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    };
+    // exclusive prefix sum of w.flag[0, n) into w.rank; *total = the sum
+    auto scan = [&](int n, int* total) -> int {
+        const int nb = (n + dt::SCAN_THREADS - 1) / dt::SCAN_THREADS;
+        dt::scan_block_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(w.flag, n, w.bsum);
+        dt::scan_top_kernel<<<1, dt::SCAN_THREADS, 0, st>>>(w.bsum, nb);
+        dt::scan_apply_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(w.flag, n, w.bsum, w.rank);
+        ctx->launches += 3;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(total, w.bsum + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    };
+    auto relocate = [&]() -> int {
+        CK(cudaMemsetAsync(w.cnt + dt::C_LEFT, 0, sizeof(unsigned), st));
+        dt::relocate_kernel<<<grid(M), 256, 0, st>>>(w, 2 * M + 16);
+        ctx->launches++;
+        return counters();
+    };
+    CK(cudaEventRecord(ctx->k0, st));
+    // validation and the seed triangle
+    CK(cudaMemsetAsync(w.cnt, 0, dt::C_N * sizeof(unsigned), st));
+    CK(cudaMemsetAsync(w.seed_key, 0xff, 8, st));
+    dt::lex_kernel<<<dt::LEX_BLOCKS, dt::LEX_THREADS, 0, st>>>(w);
+    dt::lex_final_kernel<<<1, 1, 0, st>>>(w);
+    CK(cudaGetLastError());
+    if (int rc = counters()) return rc;
+    if (cnt[dt::C_ERR]) return RTX_E_BADARG;  // non-finite or outside the predicates' domain
+    unsigned long long seed = 0;
+    dt::seed_kernel<<<grid(M), 256, 0, st>>>(w);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&seed, w.seed_key, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    ctx->launches += 3;
+    if (seed == dt::NONE) return RTX_E_BADARG;  // all points collinear
+    fill_i32_kernel<<<grid(M), 256, 0, st>>>(w.loc, M, 0);
+    dt::init_kernel<<<1, 1, 0, st>>>(w);
+    ctx->launches += 2;
+    int tcur = 4, stamp = 1;
+    if (int rc = relocate()) return rc;
+    while (cnt[dt::C_LEFT]) {
+        CK(cudaMemsetAsync(w.pick, 0xff, (size_t)tcur * 8, st));
+        CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
+        dt::pick_kernel<<<grid(M), 256, 0, st>>>(w);
+        dt::claim_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
+        dt::decide_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
+        ctx->launches += 3;
+        int added = 0;
+        if (int rc = scan(tcur, &added)) return rc;
+        int m = stamp++, s = stamp++;
+        dt::split_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m, s);
+        tcur += 2 * added;
+        dt::fix_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m);
+        ctx->launches += 2;
+        for (;;) {
+            CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
+            CK(cudaMemsetAsync(w.cnt + dt::C_FLIPS, 0, sizeof(unsigned), st));
+            const int m2 = stamp++, s2 = stamp++;
+            dt::detect_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, s);
+            dt::flip_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, s, m2, s2);
+            dt::fix_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m2);
+            ctx->launches += 3;
+            s = s2;
+            if (int rc = counters()) return rc;
+            if (!cnt[dt::C_FLIPS]) break;
+        }
+        if (int rc = relocate()) return rc;
+        if (cnt[dt::C_ERR]) return RTX_E_UNSUPPORTED;  // a broken invariant, never expected
+    }
+    // the finite triangles in slot order
+    dt::finite_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
+    ctx->launches++;
+    int nfin = 0;
+    if (int rc = scan(tcur, &nfin)) return rc;
+    dt::output_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, simplices, neighbors, (double*)transform);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, st));
+    ctx->kernel_timed = true;
+    CK(cudaStreamSynchronize(st));
+    *T = nfin;
     return 0;
 }
 

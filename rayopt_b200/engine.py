@@ -133,6 +133,26 @@ class DeviceArray:
         return v
 
 
+class DeviceTriangulation:
+    """A Delaunay triangulation in HBM (Engine.delaunay): T triangles in
+    scipy.spatial.Delaunay's layout -- simplices (T,3) int32 counter-clockwise,
+    neighbors (T,3) int32 (-1 on the hull), transform (T,3,2) FP64 -- as
+    DeviceArrays with room for 2M triangles."""
+
+    def __init__(self, T, simplices, neighbors, transform):
+        self.T = T
+        self.simplices, self.neighbors, self.transform = simplices, neighbors, transform
+
+    def free(self):
+        for a in (self.simplices, self.neighbors, self.transform):
+            a.free()
+
+    def download(self):
+        """(simplices, neighbors, transform) as numpy arrays of T rows"""
+        return tuple(a.download(np.empty((self.T,) + a.shape[1:], a.dtype))
+                     for a in (self.simplices, self.neighbors, self.transform))
+
+
 class _PinnedBlock:
     """owner of one page-locked allocation: the numpy arrays handed out by
     Engine.pinned_empty are views of its buffer, so the memory is released
@@ -703,26 +723,39 @@ class Engine:
     def grid_linear(self, points, values, tri, n, gh, download=True, winner=False):
         """rtx_grid_linear: griddata(points, values, (xs, ys), method="linear",
         fill_value=nan) on the grid node (i, j) = (gh[i], gh[j]), with the
-        host triangulation `tri` (scipy.spatial.Delaunay of `points`).
+        triangulation `tri` of `points`: scipy.spatial.Delaunay on the host,
+        or a DeviceTriangulation (``delaunay``), whose arrays are used in place;
+        `points` may be a DeviceArray, used in place too.
         Returns the (n, n) values -- numpy, or a DeviceArray when not
         `download` -- and with `winner` also the covering simplex per node
         (numpy int32, -1 where none covers it, like find_simplex)."""
-        points = np.ascontiguousarray(points, np.float64)
+        dev_points = isinstance(points, DeviceArray)
+        if not dev_points:
+            points = np.ascontiguousarray(points, np.float64)
         values = np.ascontiguousarray(values, np.float64)
         gh = np.ascontiguousarray(gh, np.float64)
-        if points.ndim != 2 or points.shape[1] != 2 or values.shape != points.shape[:1]:
-            raise ValueError("points must be (M, 2) and values (M,)")
+        if len(points.shape) != 2 or points.shape[1] != 2 or values.shape != points.shape[:1] \
+                or np.dtype(points.dtype) != np.float64:
+            raise ValueError("points must be (M, 2) FP64 and values (M,)")
         if gh.shape != (int(n),):
             raise ValueError("gh must be the (n,) grid axis")
         n = int(n)
-        simp = np.ascontiguousarray(tri.simplices, np.int32)
-        tr = np.ascontiguousarray(tri.transform, np.float64)
-        ins = [self.to_device(a) for a in (points, values, simp, tr, gh)]
+        ins = [self.to_device(a) for a in (values, gh)]
+        if not dev_points:
+            ins.append(self.to_device(points))
+        pts_ptr = points.ptr if dev_points else ins[-1].ptr
+        if isinstance(tri, DeviceTriangulation):
+            ntri, simp_ptr, tr_ptr = tri.T, tri.simplices.ptr, tri.transform.ptr
+        else:
+            simp = np.ascontiguousarray(tri.simplices, np.int32)
+            tr = np.ascontiguousarray(tri.transform, np.float64)
+            ins += [self.to_device(simp), self.to_device(tr)]
+            ntri, simp_ptr, tr_ptr = len(simp), ins[-2].ptr, ins[-1].ptr
         out = self.empty((n, n))
         win = self.empty((n, n), np.int32) if winner else None
         try:
-            check(self.lib.rtx_grid_linear(self.ctx, RTX_F64, len(points), ins[0].ptr, ins[1].ptr,
-                                           len(simp), ins[2].ptr, ins[3].ptr, n, ins[4].ptr,
+            check(self.lib.rtx_grid_linear(self.ctx, RTX_F64, points.shape[0], pts_ptr, ins[0].ptr,
+                                           ntri, simp_ptr, tr_ptr, n, ins[1].ptr,
                                            out.ptr, None if win is None else win.ptr))
             w = None
             if win is not None:
@@ -739,6 +772,51 @@ class Engine:
             for a in ins:
                 a.free()
         return (out, w) if winner else out
+
+    def selftest_predicates(self, quads):
+        """(n, 2) int: the device's exact orient2d(a, b, c) and incircle(a, b,
+        c, d) signs of n point quadruples `quads` (n, 4, 2)"""
+        q = np.ascontiguousarray(quads, np.float64).reshape(-1, 8)
+        out = np.empty((len(q), 2), np.int32)
+        check(self.lib.rtx_selftest_predicates(self.ctx, len(q), ptr(q), ptr(out)))
+        return out
+
+    def delaunay_bytes(self, m):
+        """device bytes of rtx_delaunay's workspace for m points"""
+        b = C.c_size_t()
+        check(self.lib.rtx_delaunay_bytes(self.ctx, int(m), C.byref(b)))
+        return b.value
+
+    def delaunay(self, points):
+        """rtx_delaunay: the Delaunay triangulation of `points` (M, 2) FP64,
+        numpy or a DeviceArray, computed on the device.  Returns a
+        DeviceTriangulation whose simplices, neighbors and transform stay in
+        HBM (scipy.spatial.Delaunay's layout)."""
+        if isinstance(points, DeviceArray):
+            if points.dtype != np.float64 or len(points.shape) != 2 or points.shape[1] != 2:
+                raise ValueError("points must be an (M, 2) FP64 device array")
+            dp, own = points, None
+        else:
+            a = np.ascontiguousarray(points, np.float64)
+            if a.ndim != 2 or a.shape[1] != 2:
+                raise ValueError("points must be (M, 2)")
+            dp = own = self.to_device(a)
+        m = dp.shape[0]
+        cap = max(2*m, 1)
+        simp, nbr, tr = self.empty((cap, 3), np.int32), self.empty((cap, 3), np.int32), \
+            self.empty((cap, 3, 2))
+        T = C.c_int64()
+        try:
+            check(self.lib.rtx_delaunay(self.ctx, RTX_F64, m, dp.ptr, C.byref(T), simp.ptr,
+                                        nbr.ptr, tr.ptr))
+        except Exception:
+            for a in (simp, nbr, tr):
+                a.free()
+            raise
+        finally:
+            if own is not None:
+                own.free()
+        return DeviceTriangulation(int(T.value), simp, nbr, tr)
 
     def psf_bytes(self, n, pad):
         """device bytes rtx_psf allocates for itself on an (n, n) grid"""

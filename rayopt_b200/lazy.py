@@ -415,11 +415,14 @@ class ResidentMixin:
         return x, y, t
 
     # ---- diffraction PSF with the regridding and the FFT on the device
-    def _opd_grid(self, radius, after, image, resample, download):
-        """opd's regridding on the device: the host triangulates the finite
-        exit-pupil points (scipy.spatial.Delaunay, griddata's own options),
-        rtx_grid_linear interpolates on the reference's grid"""
-        from scipy.spatial import Delaunay
+    def _opd_grid(self, radius, after, image, resample, download, triangulation="host"):
+        """opd's regridding on the device: the finite exit-pupil points are
+        triangulated on the host (scipy.spatial.Delaunay, griddata's own
+        options) or, with ``triangulation="device"``, uploaded once and
+        triangulated in HBM (rtx_delaunay); rtx_grid_linear interpolates on
+        the reference's grid"""
+        if triangulation not in ("host", "device"):
+            raise ValueError("triangulation must be 'host' or 'device', got %r" % (triangulation,))
         x, y, t = self.opd_rays(radius, after, image)
         ok = np.isfinite(x) & np.isfinite(y) & np.isfinite(t)
         x, y, t = x[ok], y[ok], t[ok]
@@ -429,28 +432,43 @@ class ResidentMixin:
         h = np.fabs((x, y)).max()
         xs, ys = np.mgrid[-1:1:1j*n, -1:1:1j*n]*h
         pts = np.stack([x, y], axis=-1)
-        o = self._engine().grid_linear(pts, t, Delaunay(pts), n, xs[:, 0].copy(),
-                                       download=download)
+        eng = self._engine()
+        if triangulation == "host":
+            from scipy.spatial import Delaunay
+            return xs, ys, eng.grid_linear(pts, t, Delaunay(pts), n, xs[:, 0].copy(),
+                                           download=download)
+        dpts = eng.to_device(pts)
+        try:
+            tri = eng.delaunay(dpts)
+            try:
+                o = eng.grid_linear(dpts, t, tri, n, xs[:, 0].copy(), download=download)
+            finally:
+                tri.free()
+        finally:
+            dpts.free()
         return xs, ys, o
 
-    def opd_device(self, radius=None, after=-2, image=-1, resample=4):
+    def opd_device(self, radius=None, after=-2, image=-1, resample=4, triangulation="host"):
         """``opd`` (rayopt/geometric_trace.py:101-144) with the regridding on
-        the device (rtx_grid_linear on the host's Delaunay triangulation):
-        griddata's values bit for bit wherever the device picks the simplex
-        scipy's find_simplex picks; nodes on shared edges may take the
-        neighbour's value (equal to rounding)"""
+        the device (rtx_grid_linear on the host's Delaunay triangulation, or
+        with ``triangulation="device"`` on rtx_delaunay's): griddata's values
+        bit for bit wherever the device picks the simplex scipy's find_simplex
+        picks; nodes on shared edges may take the neighbour's value (equal to
+        rounding)"""
         if not resample:
             return self.opd_rays(radius, after, image)
-        return self._opd_grid(radius, after, image, resample, download=True)
+        return self._opd_grid(radius, after, image, resample, download=True,
+                              triangulation=triangulation)
 
-    def psf_device(self, pad=4, resample=4, download=True, **kwargs):
+    def psf_device(self, pad=4, resample=4, download=True, triangulation="host", **kwargs):
         """``psf`` (rayopt/geometric_trace.py:146-169) on the device: the
         regridded OPD stays in HBM, the pupil function, the padded FFT
         (cuFFT) and |.|^2 run there (rtx_psf).  Returns (p, q, psf) like the
         reference; with ``download=False`` psf is a DeviceArray (free it when
         done) and ``self.psf_stats`` holds its count of finite pupil nodes,
         sum, peak and centroid sums (cp, cq) = (sum psf*p, sum psf*q) from a
-        device reduction"""
+        device reduction.  ``triangulation="device"`` triangulates the
+        exit pupil in HBM too (rtx_delaunay) instead of with scipy on the host"""
         if not resample:
             raise NotImplementedError       # as in the reference
         eng = self._engine()
@@ -458,7 +476,8 @@ class ResidentMixin:
         after, image = kwargs.pop("after", -2), kwargs.pop("image", -1)
         if kwargs:
             raise TypeError("unexpected arguments %s" % sorted(kwargs))
-        xs, ys, o = self._opd_grid(radius, after, image, resample, download=False)
+        xs, ys, o = self._opd_grid(radius, after, image, resample, download=False,
+                                   triangulation=triangulation)
         try:
             out, raw = eng.psf(o, pad)
         finally:
@@ -475,7 +494,7 @@ class ResidentMixin:
             return p, q, psf
         return p, q, out
 
-    def psf_profiles(self, pad=4, resample=4, **kwargs):
+    def psf_profiles(self, pad=4, resample=4, triangulation="host", **kwargs):
         """The encircled energy and MTF Analysis.opds (rayopt/analysis.py:
         319-346) takes from ``psf``, with the PSF kept in HBM: ``psf_device``
         (download=False), its centroid (x0, y0) = (cp, cq) from the device
@@ -484,8 +503,10 @@ class ResidentMixin:
         division: for odd sizes half a pixel from the fftshift origin, as in
         Analysis).  Returns a dict: stats, x0, y0, dx, center, xe (bin radii),
         ee (cumulative), of (frequencies) and mtf (axis 0, axis 1); the 1-d
-        inverse FFTs of the line sums run on the host."""
-        p, q, out = self.psf_device(pad, resample, download=False, **kwargs)
+        inverse FFTs of the line sums run on the host.  ``triangulation`` as
+        in ``psf_device``."""
+        p, q, out = self.psf_device(pad, resample, download=False, triangulation=triangulation,
+                                    **kwargs)
         try:
             st = self.psf_stats
             x0, y0 = st["cp"], st["cq"]

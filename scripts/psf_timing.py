@@ -10,7 +10,9 @@ staged by build() under oracle/_ref) and an H100.
 
 Device path: the per-ray OPD (rtx_trace_opd, download of x, y, t), the host
 Delaunay triangulation with its barycentric transforms, rtx_grid_linear (uploads + kernel; CUDA events give
-the kernel), rtx_psf (pupil, cuFFT, |.|^2, stats; CUDA events) and the
+the kernel), the same triangulation on the device (rtx_delaunay: the call with
+the upload of the points, its kernels by CUDA events, and whether its
+triangles are scipy's; not part of the total), rtx_psf (pupil, cuFFT, |.|^2, stats; CUDA events) and the
 download of the PSF.  Host path: griddata's evaluation on the SAME
 triangulation (LinearNDInterpolator) and the padded numpy fft2 + |.|^2.  The
 two PSFs are compared in the same run.
@@ -111,6 +113,19 @@ def main():
             t7 = time.perf_counter()
             o.free()
             out.free()
+            # the same triangulation on the device (rtx_delaunay): upload of
+            # the points and the synchronous call; CUDA events give its kernels
+            t8 = time.perf_counter()
+            dpts = eng.to_device(pts)
+            dtri = eng.delaunay(dpts)
+            t9 = time.perf_counter()
+            st["dev_triangulation_kernels_ms"] = eng.last_kernel_ms()
+            st["dev_triangulation_call_s"] = t9 - t8
+            simp = dtri.download()[0]
+            dtri.free()
+            dpts.free()
+            st["dev_triangulation_same"] = float(
+                {tuple(sorted(r)) for r in simp.tolist()} == {tuple(sorted(r)) for r in tri.simplices.tolist()})
             st.update(opd_rays_s=t1 - t0, triangulation_s=t2 - t1, regrid_call_s=t3 - t2,
                       psf_call_s=t4 - t3, profiles_call_s=t6 - t5, download_s=t7 - t6,
                       total_s=t7 - t0 - (t6 - t5))
