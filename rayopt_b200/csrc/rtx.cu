@@ -64,6 +64,7 @@ struct Tuning {
     int cluster = 1;          // CTAs per cluster of the per-CTA store kernel
     int lockstep = 1;         // CTA barrier per stored surface (STORE_WARP)
     int max_ctas_per_sm = 0;  // 0: whatever fits
+    int max_clusters = -1;    // resident clusters of the clustered kernel (-1: MAX_STORE_CLUSTERS, 0: all that fit)
     int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
 };
 
@@ -195,6 +196,12 @@ int ensure_slots(rtx_ctx* ctx, size_t bytes) {
 // of the 132 SMs; the march alone takes 1.09 ms, so the idle SMs cost less
 // than the longer runs gain).  DESIGN.md 3.7 has the whole record.
 constexpr int DEFAULT_CLUSTER = 16;
+// At most this many of those clusters run at once: fewer independent store
+// fronts write faster, and the march of 96 SMs still hides behind the stores.
+// C2 kernel on an H100 80GB HBM3 SXM at 700 W (scripts/sweep.py, medians of
+// three runs alternated): 3.52-3.53 ms with all 7 clusters that fit, 3.35-3.39
+// ms with 6 (96 CTAs).  RTX_MAX_CLUSTERS overrides it (0: all that fit).
+constexpr int MAX_STORE_CLUSTERS = 6;
 
 template <typename T, bool EXACT, int RPT, int STORE, int WARPS, int NBUF, int CLUSTER = 1>
 int launch_one(rtx_ctx* ctx, const TraceParams<T>& p, cudaStream_t stream) {
@@ -242,6 +249,8 @@ int launch_one(rtx_ctx* ctx, const TraceParams<T>& p, cudaStream_t stream) {
         }
         const long long groups = (tiles + CLUSTER - 1) / CLUSTER;
         if (ncl > groups) ncl = (int)groups;
+        const int cap = ctx->tuning.max_clusters < 0 ? MAX_STORE_CLUSTERS : ctx->tuning.max_clusters;
+        if (cap > 0 && ncl > cap) ncl = cap;
         if (ncl < 1) ncl = 1;
         cfg.gridDim = dim3((unsigned)(ncl * CLUSTER));
         ctx->last_ctas = ncl * CLUSTER;
@@ -967,6 +976,7 @@ int rtx_init(int device, rtx_ctx** out) {
         tu.tuned = true;
     if (const char* e = getenv("RTX_LOCK")) tu.lockstep = atoi(e) != 0;
     if (const char* e = getenv("RTX_MAX_CTAS")) tu.max_ctas_per_sm = atoi(e);
+    if (const char* e = getenv("RTX_MAX_CLUSTERS")) tu.max_clusters = atoi(e);
     if (const char* e = getenv("RTX_TUNE")) tu.tune = atoi(e);
     *out = ctx;
     return 0;

@@ -2,7 +2,8 @@
 """Tuning sweep of the trace kernel on the C2 workload (one wavelength bundle
 per launch, 1e7 rays, S=12, FP64): env knobs RTX_RPT / RTX_WARPS / RTX_LOCK /
 RTX_MAX_CTAS / RTX_TUNE / RTX_CLUSTER are read by rtx_init, so one Engine per
-configuration.
+configuration.  RTX_MAX_CLUSTERS (resident clusters of the clustered kernel,
+0: all that fit) is taken from the environment as set.
 usage: python scripts/sweep.py [--rays N] [--exact 0|1] cfg1 cfg2 ...
        cfg = rpt,store,warps,nbuf,lock,maxctas[,tune[,cluster]]   e.g. 2,1,8,2,1,0
        (store 1: per-warp bulk stores, 2: per-CTA bulk stores; cluster: CTAs
