@@ -49,7 +49,7 @@
 extern "C" {
 #endif
 
-#define RTX_ABI_VERSION 2
+#define RTX_ABI_VERSION 3
 
 /* maximum number of even-asphere coefficients per surface (Spheroid.aspherics,
  * elements.py:422-424).  Longer lists are rejected with RTX_E_UNSUPPORTED. */
@@ -434,33 +434,8 @@ int rtx_trace_opd(rtx_ctx *ctx, const rtx_surface *surf, int S,
 
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
- * Aimed bundle for an infinite conjugate (InfiniteConjugate.aim, rectilinear
- * projection, rayopt/conjugates.py:208-213,236-255; plane object surface) for
- * ONE field point: frame = {u[3], ybase[3], s[3], m[3]} (host, 12 doubles: the
- * common direction, yz - z*u, and the normalised sagittal / meridional
- * vectors of rayopt/utils.py:102-114), pmax = fabs(p).max() (Pupil.map,
- * rayopt/pupils.py:100).  Pupil coordinates: yp DEVICE (N,2) of `dtype`, or
- * NULL for the hexapolar grid of pupil_distribution (rayopt/utils.py:174-180)
- * with `hex_rings` rings, N = 1 + 3*hex_rings*(hex_rings+1).  Writes DEVICE
- * y0,u0 (N,3).  Asynchronous on the context stream.
- */
-int rtx_aim_infinite(rtx_ctx *ctx, int dtype, int64_t N, const void *yp,
-                     int hex_rings, const double *frame, double pmax, void *y0,
-                     void *u0);
-
-/*
- * Same for a finite conjugate (FiniteConjugate.aim, rayopt/conjugates.py:
- * 137-166; plane object surface, non-telecentric pupil, filter=False): frame =
- * {y[3] object point, u[3] = (0,0,z) - y, s[3], m[3]}, am = max |arctan2(p, z)|
- * (the pupil half-angle Pupil.map scales with), z the pupil distance.
- */
-int rtx_aim_finite(rtx_ctx *ctx, int dtype, int64_t N, const void *yp,
-                   int hex_rings, const double *frame, double am, double z,
-                   void *y0, void *u0);
-
-/*
- * General generator: the pupil grids of pupil_distribution (rayopt/utils.py:
- * 118-199), Pupil.map with its elliptical filter (rayopt/pupils.py:97-107) and
+ * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map
+ * with its elliptical filter (rayopt/pupils.py:97-107) and
  * Conjugate.aim (rayopt/conjugates.py:137-166, 236-255) evaluated per ray on
  * the device.  Candidates rejected by a predicate (mesh points outside the
  * unit circle, rays outside the filter ellipse) are squeezed out in order

@@ -61,8 +61,6 @@ SYMBOLS = {
     "rtx_trace_opd": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
-    "rtx_aim_infinite": (_i, [_vp, _i, _i64, _vp, _i, _vp, C.c_double, _vp, _vp]),
-    "rtx_aim_finite": (_i, [_vp, _i, _i64, _vp, _i, _vp, C.c_double, C.c_double, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),
     "rtx_aim_rays": (_i, [_vp, _vp, _i64, _vp, _i, _i64, _i64, _vp, _vp, _vp]),
     "rtx_focus_moments": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),

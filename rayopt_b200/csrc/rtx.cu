@@ -1670,54 +1670,6 @@ int rtx_trace_opd(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* ro
     return 0;
 }
 
-int rtx_aim_infinite(rtx_ctx* ctx, int dtype, int64_t N, const void* yp, int hex_rings,
-                     const double* frame, double pmax, void* y0, void* u0) {
-    if (!ctx || !frame || !y0 || !u0 || N < 0) return RTX_E_BADARG;
-    if (!yp && (hex_rings < 0 || N != 1 + 3ll * hex_rings * (hex_rings + 1))) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
-    long long blocks = (N + 255) / 256;
-    long long cap = (long long)ctx->sm_count * 16;
-    if (blocks > cap) blocks = cap;
-    const double* f = frame;
-    if (dtype == RTX_F64)
-        aim_infinite_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-            (const double*)yp, hex_rings, N, pmax, f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7],
-            f[8], f[9], f[10], f[11], (double*)y0, (double*)u0);
-    else if (dtype == RTX_F32)
-        aim_infinite_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-            (const float*)yp, hex_rings, N, pmax, f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7],
-            f[8], f[9], f[10], f[11], (float*)y0, (float*)u0);
-    else
-        return RTX_E_BADARG;
-    ctx->launches++;
-    return (int)cudaGetLastError();
-}
-
-int rtx_aim_finite(rtx_ctx* ctx, int dtype, int64_t N, const void* yp, int hex_rings,
-                   const double* frame, double am, double z, void* y0, void* u0) {
-    if (!ctx || !frame || !y0 || !u0 || N < 0) return RTX_E_BADARG;
-    if (!yp && (hex_rings < 0 || N != 1 + 3ll * hex_rings * (hex_rings + 1))) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
-    long long blocks = (N + 255) / 256;
-    long long cap = (long long)ctx->sm_count * 16;
-    if (blocks > cap) blocks = cap;
-    const double* f = frame;
-    if (dtype == RTX_F64)
-        aim_finite_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-            (const double*)yp, hex_rings, N, am, z, f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7],
-            f[8], f[9], f[10], f[11], (double*)y0, (double*)u0);
-    else if (dtype == RTX_F32)
-        aim_finite_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-            (const float*)yp, hex_rings, N, am, z, f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7],
-            f[8], f[9], f[10], f[11], (float*)y0, (float*)u0);
-    else
-        return RTX_E_BADARG;
-    ctx->launches++;
-    return (int)cudaGetLastError();
-}
-
 }  // extern "C"
 
 namespace {

@@ -72,6 +72,16 @@ def _check_trace_operands(dtype, N, rows, ld, outputs, mask=None, path_sum=None)
                              % (N, words, mask.nbytes//4))
 
 
+def _given(yp):
+    """(n_given, pointer) of the DEVICE pupil coordinates of a GRID_GIVEN
+    bundle, which the generator reads as (n, 2) FP64 whatever the rays' type"""
+    if yp is None:
+        return 0, None
+    if np.dtype(yp.dtype) != np.float64:
+        raise ValueError("given pupil coordinates must be float64, got %s" % np.dtype(yp.dtype))
+    return yp.shape[0], yp.ptr
+
+
 class DeviceArray:
     """A typed block of HBM owned by an Engine (freed with it or on .free())."""
 
@@ -574,39 +584,23 @@ class Engine:
 
     def aim_infinite_device(self, yo, z, p, angle, yp=None, nrays=None, dtype=np.float64,
                             rings=None):
-        """Launch rays of an aimed bundle generated in HBM (rtx_aim_infinite):
-        `yp` a DEVICE (N,2) array of pupil coordinates, or None for the
-        hexapolar grid with about `nrays` rays (or exactly `rings` rings).
-        Returns DeviceArrays (y0, u0)."""
-        from .rays import aim_frame
-        frame = np.ascontiguousarray(np.concatenate(aim_frame(yo, z, angle)), np.float64)
-        pmax = float(np.fabs(np.asarray(p, float)).max())
-        if yp is None:
-            if rings is None:
-                rings = int(np.sqrt(nrays/3. - 1/12.) - 1/2.)
-            N = 1 + 3*rings*(rings + 1)
-        else:
-            rings, N = 0, yp.shape[0]
-        y0, u0 = self.empty((N, 3), dtype), self.empty((N, 3), dtype)
-        check(self.lib.rtx_aim_infinite(self.ctx, _code(dtype), N, None if yp is None else yp.ptr,
-                                        rings, ptr(frame), pmax, y0.ptr, u0.ptr))
-        return y0, u0
+        """Launch rays of an aimed bundle for an infinite object (rectilinear
+        projection, plane object surface) generated in HBM: `yp` a DEVICE
+        (N,2) FP64 array of pupil coordinates, or None for the hexapolar grid
+        with about `nrays` rays (or exactly `rings` rings).  Host
+        restatement: rays.aim_infinite.  Returns DeviceArrays (y0, u0)."""
+        from .rays import infinite_record, pupil_grid
+        return self.aim_rays(infinite_record(yo, z, p, angle, grid=pupil_grid(yp, nrays, rings)),
+                             dtype, yp=yp)
 
     def aim_finite_device(self, yo, z, p, radius, yp=None, nrays=None, dtype=np.float64):
-        """Launch rays of an aimed bundle from a FINITE object generated in HBM
-        (rtx_aim_finite; host restatement: rays.aim_finite).  Returns (y0, u0)."""
-        from .rays import finite_frame
-        frame = np.ascontiguousarray(np.concatenate(finite_frame(yo, z, radius)), np.float64)
-        am = float(np.fabs(np.arctan2(np.asarray(p, float), z)).max())
-        if yp is None:
-            rings = int(np.sqrt(nrays/3. - 1/12.) - 1/2.)
-            N = 1 + 3*rings*(rings + 1)
-        else:
-            rings, N = 0, yp.shape[0]
-        y0, u0 = self.empty((N, 3), dtype), self.empty((N, 3), dtype)
-        check(self.lib.rtx_aim_finite(self.ctx, _code(dtype), N, None if yp is None else yp.ptr,
-                                      rings, ptr(frame), am, float(z), y0.ptr, u0.ptr))
-        return y0, u0
+        """Launch rays of an aimed bundle from a FINITE object (non-telecentric
+        pupil, plane object surface) generated in HBM, `yp` and `nrays` as in
+        aim_infinite_device.  Host restatement: rays.aim_finite.  Returns
+        (y0, u0)."""
+        from .rays import finite_record, pupil_grid
+        return self.aim_rays(finite_record(yo, z, p, radius, grid=pupil_grid(yp, nrays)),
+                             dtype, yp=yp)
 
     def aim_rays(self, spec, dtype=np.float64, first=0, count=None, yp=None, want_pupil=False):
         """rtx_aim_plan + rtx_aim_rays: launch rays `first .. first+count-1` of
@@ -615,8 +609,7 @@ class Engine:
         Returns (y0, u0) DeviceArrays, plus the (count,2) pupil coordinates
         when `want_pupil`."""
         spec = np.ascontiguousarray(spec)
-        n_given = 0 if yp is None else yp.shape[0]
-        ypp = None if yp is None else yp.ptr
+        n_given, ypp = _given(yp)
         total = C.c_int64()
         check(self.lib.rtx_aim_plan(self.ctx, ptr(spec), n_given, ypp, C.byref(total)))
         count = total.value - first if count is None else int(count)
@@ -629,24 +622,17 @@ class Engine:
     def aim_rays_into(self, spec, y_dst, u_dst, count, first=0, yp=None):
         """rtx_aim_rays into existing device rows (DeviceArray views)"""
         spec = np.ascontiguousarray(spec)
-        check(self.lib.rtx_aim_rays(self.ctx, ptr(spec), 0 if yp is None else yp.shape[0],
-                                    None if yp is None else yp.ptr, _code(y_dst.dtype), int(first),
-                                    int(count), y_dst.ptr, u_dst.ptr, None))
+        n_given, ypp = _given(yp)
+        check(self.lib.rtx_aim_rays(self.ctx, ptr(spec), n_given, ypp, _code(y_dst.dtype),
+                                    int(first), int(count), y_dst.ptr, u_dst.ptr, None))
 
     def aim_count(self, spec, yp=None):
         """number of rays the record generates (after clipping / filtering)"""
         spec = np.ascontiguousarray(spec)
+        n_given, ypp = _given(yp)
         total = C.c_int64()
-        check(self.lib.rtx_aim_plan(self.ctx, ptr(spec), 0 if yp is None else yp.shape[0],
-                                    None if yp is None else yp.ptr, C.byref(total)))
+        check(self.lib.rtx_aim_plan(self.ctx, ptr(spec), n_given, ypp, C.byref(total)))
         return total.value
-
-    def aim_infinite_into(self, y_dst, u_dst, count, rings, frame, pmax, yp=None):
-        """rtx_aim_infinite into existing device rows (DeviceArray views)"""
-        frame = np.ascontiguousarray(frame, np.float64)
-        check(self.lib.rtx_aim_infinite(self.ctx, _code(y_dst.dtype), int(count),
-                                        None if yp is None else yp.ptr, int(rings), ptr(frame),
-                                        float(pmax), y_dst.ptr, u_dst.ptr))
 
     def selftest_math(self, a, b):
         """(6, n): engine a/b, IEEE a/b, engine sqrt(a), IEEE sqrt(a),

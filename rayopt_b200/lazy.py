@@ -541,27 +541,27 @@ class ResidentTrace(ResidentMixin):
 
     def rays_infinite(self, yo, z, p, angle, l=None, nrays=None, yp=None, ref=0):
         """Launch rays of an aimed bundle for an infinite conjugate generated
-        directly in HBM (Engine.aim_infinite_device / rtx_aim_infinite): the
-        hexapolar grid with about `nrays` rays, or the DEVICE pupil coordinates
-        `yp` (N,2); (z, p) is the reference's pupil-aiming solution
-        (System.pupil).  Nothing crosses PCIe."""
-        from .rays import aim_frame
+        directly in HBM (as Engine.aim_infinite_device): the hexapolar grid
+        with about `nrays` rays, or the DEVICE FP64 pupil coordinates `yp`
+        (N,2); (z, p) is the reference's pupil-aiming solution (System.pupil).
+        Nothing crosses PCIe."""
+        from .rays import infinite_record, pupil_grid
+        spec = infinite_record(yo, z, p, angle, grid=pupil_grid(yp, nrays))
+        self._generate(spec, yp, self.system.wavelengths[0] if l is None else l, ref)
+
+    def _generate(self, spec, yp, l, ref):
+        """the bundle of the `rtx_aim` record `spec` into row 0, at wavelength
+        `l` with default weights and reference ray `ref`"""
         eng = self.engine
-        if yp is None:
-            rings = int(np.sqrt(nrays/3. - 1/12.) - 1/2.)
-            count = 1 + 3*rings*(rings + 1)
-        else:
-            rings, count = 0, yp.shape[0]
+        count = eng.aim_count(spec, yp)
         if self._dev is None or self.nrays != count:
             self.allocate(count)
-        self.l = self.system.wavelengths[0] if l is None else l
+        self.l = l
         self.w = None
         self._w_default, self._w_dev = True, None
         self.ref = ref
-        frame = np.concatenate(aim_frame(yo, z, angle))
-        pmax = float(np.fabs(np.asarray(p, float)).max())
         d = self._dev
-        eng.aim_infinite_into(d["y"].rows(0), d["u"].rows(0), count, rings, frame, pmax, yp)
+        eng.aim_rays_into(spec, d["y"].rows(0), d["u"].rows(0), count, yp=yp)
         d["i"].rows(0).copy_from(d["u"].rows(0), count*24)   # i[0] = u[0] (geometric_trace.py:68)
         self._zero_t0()
         for a in (self.y, self.u, self.i, self.t):
@@ -578,27 +578,13 @@ class ResidentTrace(ResidentMixin):
         surfaces.  ``system.pupil`` (the aiming) stays host Python.  Returns
         False (nothing done) for the distributions that stay on the host."""
         from .rays import aim_record, grid_spec
-        s, eng = self.system, self.engine
+        s = self.system
         ref, grid = grid_spec(distribution, nrays)
         if grid is None:
             return False
         l = s.wavelengths[0] if wavelength is None else wavelength
         z, p = s.pupil(yo, l=wavelength, stop=stop)
-        spec = aim_record(s.object, yo, z, p, grid, filter, s[0], seed)
-        count = eng.aim_count(spec)
-        if self._dev is None or self.nrays != count:
-            self.allocate(count)
-        self.l = l
-        self.w = None
-        self._w_default, self._w_dev = True, None
-        self.ref = ref
-        d = self._dev
-        eng.aim_rays_into(spec, d["y"].rows(0), d["u"].rows(0), count)
-        d["i"].rows(0).copy_from(d["u"].rows(0), count*24)   # i[0] = u[0] (geometric_trace.py:68)
-        self._zero_t0()
-        for a in (self.y, self.u, self.i, self.t):
-            a.invalidate()
-        self.n[0] = s.refractive_index(self.l, 0)
+        self._generate(aim_record(s.object, yo, z, p, grid, filter, s[0], seed), None, l, ref)
         return True
 
     def rays_point(self, yo, wavelength=None, nrays=11, distribution="hexapolar",

@@ -1,5 +1,6 @@
-"""Launch-ray generation for aimed bundles (host numpy restatements; the device
-kernels rtx_aim_infinite / rtx_aim_finite follow them operation by operation).
+"""Launch-ray generation for aimed bundles: host numpy restatements, which the
+tests and the benchmark compare the device generator (rtx_aim_rays) against,
+and the per-field `rtx_aim` records that generator reads.
 
 Restates, for the cases the benchmark workloads need, what the reference does
 upstream of the hot path:  ``InfiniteConjugate.aim`` with the rectilinear
@@ -49,25 +50,6 @@ def hexapolar_xy(idx, rings):
     return xy
 
 
-def aim_frame(yo, z, angle):
-    """The per-field constants of aim_infinite: (u, ybase, s, m), each (3,):
-    the common ray direction, yz - z*u, and the normalised sagittal and
-    meridional pupil axes."""
-    yo = np.atleast_2d(np.asarray(yo, float))
-    yt = yo*np.tan(angle)
-    u = np.hstack((yt, np.ones((1, 1))))
-    u /= np.sqrt(np.square(u).sum(-1))[:, None]
-    yz = np.array((0, 0, z), float)
-    ybase = yz - z*u
-    s = np.cross(u, yz)
-    if np.all(s == 0):
-        s = np.array([[1., 0, 0]])
-    m = np.cross(u, s)
-    s = s/np.sqrt(np.square(s).sum(-1))[..., None]
-    m = m/np.sqrt(np.square(m).sum(-1))[..., None]
-    return u[0], ybase[0], s[0], m[0]
-
-
 def aim_infinite(yo, yp, z, p, angle):
     """Rays (y, u), each (N, 3), for fractional object coordinate `yo` (2,),
     fractional pupil coordinates `yp` (N, 2), pupil distance `z`, pupil
@@ -94,20 +76,19 @@ def aim_infinite(yo, yp, z, p, angle):
     return y, u
 
 
-def finite_frame(yo, z, radius):
-    """Per-field constants of aim_finite: object point y (3,), chief direction
-    u = (0,0,z) - y (3,), normalised sagittal and meridional axes s, m (3,)."""
+def finite_frame(yo, z, radius, telecentric=False, surface=None):
+    """Per-field constants of FiniteConjugate.aim: object point y (3,), chief
+    direction u = (0,0,z) - y, or (0,0,z) for a `telecentric` pupil (3,),
+    normalised sagittal and meridional axes s, m (3,).  `surface`: a curved
+    object surface, on which the object point lies."""
     yo = np.atleast_2d(np.asarray(yo, float))
     y = np.zeros((1, 3))
     y[..., :2] = -yo*radius                                # conjugates.py:151
+    if surface is not None:
+        y[..., 2] = -surface.surface_sag(y)                # :153
     uz = np.array((0, 0, z), float)
-    u = uz - y                                             # conjugates.py:158
-    s = np.cross(u, uz)
-    if np.all(s == 0):
-        s = np.array([[1., 0, 0]])
-    m = np.cross(u, s)
-    s = s/np.sqrt(np.square(s).sum(-1))[..., None]
-    m = m/np.sqrt(np.square(m).sum(-1))[..., None]
+    u = np.tile(uz, (1, 1)) if telecentric else uz - y    # :155-158
+    s, m = _sagittal_meridional(u, uz)
     return y[0], u[0], s[0], m[0]
 
 
@@ -183,6 +164,18 @@ def grid_spec(distribution, nrays):
     raise ValueError("unknown ray distribution", d)
 
 
+def pupil_grid(yp, nrays=None, rings=None):
+    """`grid` of a bundle whose pupil coordinates are the device array `yp`
+    (None: GRID_GIVEN), or else of the hexapolar grid with `rings` rings or
+    about `nrays` rays"""
+    if yp is not None:
+        return None
+    if rings is None:
+        _, g = grid_spec("hexapolar", nrays)
+        rings = 0 if g is None else g["n"]       # one ray: the axial ray alone
+    return dict(grid=GRID_HEXAPOLAR, n=rings)
+
+
 def project(yo, angle, projection="rectilinear"):
     """InfiniteConjugate.map (rayopt/conjugates.py:208-234): field -> direction"""
     yo = np.atleast_2d(np.asarray(yo, float))
@@ -228,39 +221,18 @@ def _sagittal_meridional(u, z):
     return s, m
 
 
-def aim_record(obj, yo, z, p, grid=None, filter=False, surface=None, seed=0):
-    """One `rtx_aim` record for field point `yo` of a rayopt conjugate `obj`
-    (``system.object``: InfiniteConjugate or FiniteConjugate, duck-typed) with
-    the pupil-aiming solution ``(z, p)`` of ``System.pupil``; `grid` from
-    grid_spec() (None: pupil coordinates are given), `surface` = ``system[0]``."""
-    from .surface_table import pack_element
+def _curved(surface):
+    return surface is not None and (getattr(surface, "curvature", 0.) or
+                                    getattr(surface, "aspherics", None) is not None)
+
+
+def _record(conjugate, frame, a, z, grid, filter, seed):
+    """the `rtx_aim` record of one field point with pupil half-apertures (or,
+    finite, half-angles) `a` (2, 2)"""
     rec = np.zeros(1, aim_dtype())
     r = rec[0]
-    yo = np.atleast_2d(np.asarray(yo, float))
-    a = np.asarray(p, float).reshape(2, 2)
-    curved_surface = surface is not None and (getattr(surface, "curvature", 0.) or
-                                              getattr(surface, "aspherics", None) is not None)
-    if getattr(obj, "finite", False):
-        r["conjugate"] = 1
-        a = np.arctan2(a, z)                               # conjugates.py:146
-        y = np.zeros((1, 3))
-        y[..., :2] = -yo*obj.radius                        # :151
-        if surface is not None and curved_surface:
-            y[..., 2] = -surface.surface_sag(y)            # :153
-        uz = np.array((0, 0, z), float)
-        u = np.tile(uz, (1, 1)) if obj.pupil.telecentric else uz - y   # :155-158
-        s, m = _sagittal_meridional(u, uz)
-        r["frame"] = np.concatenate((y[0], u[0], s[0], m[0]))
-    else:
-        r["conjugate"] = 0
-        u = project(yo, obj.angle, getattr(obj, "projection", "rectilinear"))
-        yz = np.array((0, 0, z), float)
-        s, m = _sagittal_meridional(u, yz)
-        r["frame"] = np.concatenate((u[0], (yz - z*u)[0], s[0], m[0]))   # :249
-        if curved_surface:
-            from .elements import _Bare
-            r["curved"] = 1
-            pack_element(r["surface"], _Bare(surface, mu=1.), 1., None)
+    r["conjugate"] = conjugate
+    r["frame"] = np.concatenate(frame)
     r["pmax"] = np.fabs(a).max()                           # pupils.py:100
     r["z"] = z
     r["filter"] = int(bool(filter))
@@ -273,3 +245,43 @@ def aim_record(obj, yo, z, p, grid=None, filter=False, surface=None, seed=0):
     r["seg"] = g.get("seg", np.zeros((2, 4)))
     r["seg_m"] = g.get("seg_m", (0, 0))
     return rec
+
+
+def infinite_record(yo, z, p, angle, projection="rectilinear", grid=None, filter=False,
+                    surface=None, seed=0):
+    """`rtx_aim` record of InfiniteConjugate.aim (conjugates.py:236-255) for
+    field point `yo` of an object at semi-angle `angle` in `projection`;
+    frame (u, ybase = yz - z*u, s, m)"""
+    u = project(yo, angle, projection)
+    yz = np.array((0, 0, z), float)
+    s, m = _sagittal_meridional(u, yz)
+    frame = u[0], (yz - z*u)[0], s[0], m[0]                # :249
+    rec = _record(0, frame, np.asarray(p, float).reshape(2, 2), z, grid, filter, seed)
+    if _curved(surface):
+        from .elements import _Bare
+        from .surface_table import pack_element
+        r = rec[0]
+        r["curved"] = 1
+        pack_element(r["surface"], _Bare(surface, mu=1.), 1., None)
+    return rec
+
+
+def finite_record(yo, z, p, radius, telecentric=False, grid=None, filter=False, surface=None,
+                  seed=0):
+    """`rtx_aim` record of FiniteConjugate.aim (conjugates.py:137-166) for
+    field point `yo` of an object of `radius`; frame as finite_frame"""
+    a = np.arctan2(np.asarray(p, float).reshape(2, 2), z)  # conjugates.py:146
+    frame = finite_frame(yo, z, radius, telecentric, surface if _curved(surface) else None)
+    return _record(1, frame, a, z, grid, filter, seed)
+
+
+def aim_record(obj, yo, z, p, grid=None, filter=False, surface=None, seed=0):
+    """One `rtx_aim` record for field point `yo` of a rayopt conjugate `obj`
+    (``system.object``: InfiniteConjugate or FiniteConjugate, duck-typed) with
+    the pupil-aiming solution ``(z, p)`` of ``System.pupil``; `grid` from
+    grid_spec() (None: pupil coordinates are given), `surface` = ``system[0]``."""
+    if getattr(obj, "finite", False):
+        return finite_record(yo, z, p, obj.radius, obj.pupil.telecentric, grid, filter, surface,
+                             seed)
+    return infinite_record(yo, z, p, obj.angle, getattr(obj, "projection", "rectilinear"), grid,
+                           filter, surface, seed)

@@ -6,7 +6,7 @@ every GPU.  Under torchrun, one rank per GPU:
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         --master-port 29561 tests/gpu_scripts/c4_spot.py [rays_per_rank]
 
-Every rank generates its shard in HBM (rtx_aim_infinite, hexapolar pupil grid,
+Every rank generates its shard in HBM (rtx_aim_rays, hexapolar pupil grid,
 its own field point), marches it through the 12 surfaces and the SAME kernel
 bulk-stores y[-1] into the gather buffers of all ranks over NVLink
 (rtx_trace_gather) -- no NCCL in the data path.  A sample of a PEER's segment

@@ -31,8 +31,11 @@ def test_header_symbols_all_exported(lib):
         assert hasattr(raw, name), name
 
 
-def test_abi_version_and_layout(lib):
-    assert lib.rtx_abi_version() == 2
+def test_abi_version_matches_header_and_layout(lib):
+    """version 3: the library reports the version include/rtx.h declares"""
+    text = open(os.path.join(ROOT, "include", "rtx.h")).read()
+    declared = int(re.search(r"#define\s+RTX_ABI_VERSION\s+(\d+)", text).group(1))
+    assert lib.rtx_abi_version() == declared == 3
     assert lib.rtx_sizeof_surface() == SURFACE_DTYPE.itemsize
     from rayopt_b200.engine import OPD_DTYPE
     from rayopt_b200.rays import aim_dtype
@@ -40,13 +43,13 @@ def test_abi_version_and_layout(lib):
     assert lib.rtx_sizeof_aim() == aim_dtype().itemsize     # struct rtx_aim
 
 
-def test_selftest_math2_rejects_bad_arguments(lib):
+def test_selftest_math2_refuses_bad_arguments(lib):
     """the primitives' self-test entry point checks its arguments before any
-    device work (ABI version unchanged: a new symbol, no changed one)"""
+    device work (ABI version 3)"""
     a = np.ones(4)
     p = a.ctypes.data_as(C.c_void_p)
     assert lib.rtx_selftest_math2(None, 4, p, p, p, p) == -1         # RTX_E_BADARG
-    assert lib.rtx_abi_version() == 2
+    assert lib.rtx_abi_version() == 3
 
 
 def test_strerror(lib):

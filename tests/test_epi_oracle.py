@@ -206,6 +206,33 @@ def test_engine_refuses_mismatched_operands():
                 call()
 
 
+def test_aim_refuses_given_pupil_coordinates_not_fp64():
+    """the ray generator reads given pupil coordinates as FP64 for FP64 and
+    FP32 bundles alike: an array of another type raises ValueError before the
+    library is called"""
+    from rayopt_b200.engine import Engine
+    from rayopt_b200.rays import infinite_record
+    eng = object.__new__(Engine)
+    eng.lib, eng.ctx = _NoLib(), None
+    p = np.array(((-3., -2.5), (2., 2.8)))
+    rec = infinite_record((0, .5), 30., p, .2)
+    y = _dev((100, 3), np.float32)
+    for dt in (np.float32, np.float16):
+        yp = _dev((100, 2), dt)
+        bad = [
+            lambda: eng.aim_infinite_device((0, .5), 30., p, .2, yp=yp, dtype=np.float32),
+            lambda: eng.aim_finite_device((0, .5), 30., p, 5., yp=yp),
+            lambda: eng.aim_rays(rec, yp=yp),
+            lambda: eng.aim_rays_into(rec, y, y, 100, yp=yp),
+            lambda: eng.aim_count(rec, yp),
+        ]
+        for call in bad:
+            with pytest.raises(ValueError):
+                call()
+    with pytest.raises(AssertionError, match="called"):
+        eng.aim_count(rec, _dev((100, 2), np.float64))
+
+
 def test_trace_device_refuses_mismatched_operands():
     """Engine.trace_device, trace_device_batch and trace_gather: an output or
     path sum of another dtype than the rays, an output smaller than rows x ld

@@ -588,7 +588,7 @@ def test_resident_trace_lazy_rows(eng, systems):
 
 
 def test_device_ray_generation(eng, systems):
-    """rtx_aim_infinite: launch rays generated in HBM equal the host
+    """aim_infinite_device: launch rays generated in HBM equal the host
     restatement of InfiniteConjugate.aim (rayopt_b200/rays.py, itself
     bit-identical to the reference): bit for bit for given pupil coordinates,
     to the last ulps of sin/cos for the on-the-fly hexapolar grid; traced, they
@@ -690,7 +690,7 @@ def test_batched_bundles_one_launch(eng, systems, dtype):
 
 
 def test_device_ray_generation_finite(eng):
-    """rtx_aim_finite vs the host restatement of FiniteConjugate.aim (which is
+    """aim_finite_device vs the host restatement of FiniteConjugate.aim (which is
     bit-identical to the reference): to the last ulps of tan()"""
     from rayopt_b200.rays import aim_finite, hexapolar
     p = np.array(((-3., -2.5), (3., 2.5)))
