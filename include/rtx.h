@@ -432,6 +432,52 @@ int rtx_trace_opd(rtx_ctx *ctx, const rtx_surface *surf, int S,
                   const void *u0, int clip, const rtx_opd *opd, void *A,
                   void *P, unsigned flags);
 
+/*
+ * Through-focus spot images (Analysis.spots, rayopt/analysis.py:250-283) as
+ * integer histograms.  For each ray and plane k < planes, in FP64 with every
+ * operation separately rounded (FP32 rays are widened first):
+ *   d = y_xy - c,  u = i_xy / i_z,  q = (d + z[k] u) - o[k]
+ *   radial = 0: (q_x, q_y) binned as np.histogram2d(qx, qy, (nx, ny), range)
+ *   radial = 1: r = sqrt(q_x^2 + q_y^2) binned as np.histogram(r, nx, range[0])
+ * Binning: edges e_j = j*step + lo, step = (hi - lo)/n, e_n = hi
+ * (np.linspace); bin = searchsorted(e, x, "right") - 1 with x == hi in the
+ * last bin; points outside [lo, hi], NaN and +-inf are not counted.
+ *
+ * counts: DEVICE uint64 (planes, nx, ny) (radial: (planes, nx)), ADDED to (the
+ * caller zeroes it), or NULL.  tally: host (planes, 2) uint64 = rays binned,
+ * rays with a non-finite q.  extent: host (planes, 3) doubles = max |q_x|,
+ * max |q_y|, max r over the rays with a finite q (0 when there is none).
+ * Counts, tallies and extents are exact, so they are the same in every call,
+ * context and chunking of a bundle, and chunks add up.
+ *
+ * RTX_E_BADARG, before any device work, for planes outside 1..16, nx or ny
+ * < 1, ny != 1 in radial mode, planes*nx*ny >= 2^31, a non-finite range end,
+ * lo >= hi, a step (hi - lo)/n that is not a normal number, a non-finite z
+ * or o, or counts and extent both NULL.  N = 0 adds nothing.
+ */
+#define RTX_SPOT_MAX_PLANES 16
+typedef struct rtx_spot {
+    int32_t planes, radial;           /* K in 1..16; 0: 2-D image, 1: radial */
+    int64_t nx, ny;                   /* bins (radial: nx; ny must be 1) */
+    double range[2][2];               /* [[x_lo, x_hi], [y_lo, y_hi]]; radial: range[0] */
+    double c[2];                      /* subtracted from y_xy first (the chief ray's) */
+    double z[RTX_SPOT_MAX_PLANES];    /* defocus distances */
+    double o[RTX_SPOT_MAX_PLANES][2]; /* per-plane offsets subtracted last */
+} rtx_spot;
+size_t rtx_sizeof_spot(void);
+/* the march to surface S-1 (as rtx_trace_reduce) with the binning as its
+ * epilogue: nothing per ray is stored.  Synchronous. */
+int rtx_trace_spot(rtx_ctx *ctx, const rtx_surface *surf, int S,
+                   const double *rot0, int dtype, int64_t N, const void *y0,
+                   const void *u0, int clip, const rtx_spot *spot,
+                   uint64_t *counts, uint64_t *tally, double *extent,
+                   unsigned flags);
+/* the same binning of stored rows: y, inc DEVICE (N,3) of dtype (a trace's
+ * y[at] and i[at]).  Synchronous. */
+int rtx_spot_rows(rtx_ctx *ctx, int dtype, int64_t N, const void *y,
+                  const void *inc, const rtx_spot *spot, uint64_t *counts,
+                  uint64_t *tally, double *extent);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

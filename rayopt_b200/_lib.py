@@ -22,6 +22,7 @@ SYMBOLS = {
     "rtx_sizeof_surface": (_sz, []),
     "rtx_sizeof_aim": (_sz, []),
     "rtx_sizeof_opd": (_sz, []),
+    "rtx_sizeof_spot": (_sz, []),
     "rtx_device_count": (_i, []),
     "rtx_strerror": (C.c_char_p, [_i]),
     "rtx_surface_finalize": (_i, [_vp, _i, _vp]),
@@ -59,6 +60,8 @@ SYMBOLS = {
     "rtx_moments": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp]),
     "rtx_trace_reduce": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_opd": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),
+    "rtx_trace_spot": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _vp, _u]),
+    "rtx_spot_rows": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),
@@ -107,6 +110,10 @@ def load():
     if lib.rtx_sizeof_aim() != aim_dtype().itemsize:
         raise RtxError("rtx_aim layout mismatch: C %d, numpy %d" % (
             lib.rtx_sizeof_aim(), aim_dtype().itemsize))
+    from .engine import SPOT_DTYPE
+    if lib.rtx_sizeof_spot() != SPOT_DTYPE.itemsize:
+        raise RtxError("rtx_spot layout mismatch: C %d, numpy %d" % (
+            lib.rtx_sizeof_spot(), SPOT_DTYPE.itemsize))
     _lib = lib
     return lib
 

@@ -84,6 +84,7 @@ struct rtx_ctx {
     ChunkBuf chunk[2];
     double* d_moments = nullptr;
     double* d_epi = nullptr;  // rtx_trace_reduce
+    unsigned long long* d_spot = nullptr;  // rtx_trace_spot / rtx_spot_rows: tallies, extents
     // cached plan of the ray generator (rtx_aim_plan / rtx_aim_rays)
     std::vector<unsigned char> aim_key;
     std::vector<long long> aim_offsets;  // per block; empty: nothing is rejected
@@ -886,6 +887,7 @@ int rtx_abi_version(void) { return RTX_ABI_VERSION; }
 size_t rtx_sizeof_surface(void) { return sizeof(rtx_surface); }
 size_t rtx_sizeof_aim(void) { return sizeof(rtx_aim); }
 size_t rtx_sizeof_opd(void) { return sizeof(rtx_opd); }
+size_t rtx_sizeof_spot(void) { return sizeof(rtx_spot); }
 
 int rtx_device_count(void) {
     int n = 0;
@@ -996,6 +998,7 @@ int rtx_free(rtx_ctx* ctx) {
     free_chunk(ctx->chunk[1]);
     if (ctx->d_moments) cudaFree(ctx->d_moments);
     if (ctx->d_epi) cudaFree(ctx->d_epi);
+    if (ctx->d_spot) cudaFree(ctx->d_spot);
     if (ctx->d_aim_offsets) cudaFree(ctx->d_aim_offsets);
     if (ctx->d_winner) cudaFree(ctx->d_winner);
     release_fft_plan(ctx);
@@ -1668,6 +1671,140 @@ int rtx_trace_opd(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* ro
     CK(cudaEventRecord(ctx->k1, ctx->stream));
     ctx->kernel_timed = true;
     return 0;
+}
+
+}  // extern "C"
+
+namespace {
+// rtx_spot -> SpotDev with every check include/rtx.h lists (host only: no
+// device work before a refusal)
+int spot_to_dev(const rtx_spot* s, const uint64_t* counts, const double* extent, SpotDev& d) {
+    if (!s || (!counts && !extent)) return RTX_E_BADARG;
+    if (s->planes < 1 || s->planes > RTX_SPOT_MAX_PLANES) return RTX_E_BADARG;
+    if (s->radial != 0 && s->radial != 1) return RTX_E_BADARG;
+    if (s->nx < 1 || s->ny < 1 || (s->radial && s->ny != 1)) return RTX_E_BADARG;
+    const long long lim = 1LL << 31;
+    if (s->nx >= lim || s->ny >= lim) return RTX_E_BADARG;
+    const long long kn = (long long)s->planes * s->nx;
+    if (kn >= lim || kn * s->ny >= lim) return RTX_E_BADARG;
+    memset(&d, 0, sizeof(d));
+    d.K = s->planes;
+    d.radial = s->radial;
+    d.nx = (int)s->nx;
+    d.ny = (int)s->ny;
+    for (int a = 0; a < (s->radial ? 1 : 2); ++a) {
+        const double lo = s->range[a][0], hi = s->range[a][1];
+        if (!std::isfinite(lo) || !std::isfinite(hi) || !(lo < hi)) return RTX_E_BADARG;
+        const double n = (double)(a == 0 ? s->nx : s->ny);
+        const double step = (hi - lo) / n;  // np.linspace's step
+        if (!std::isnormal(step)) return RTX_E_BADARG;
+        d.lo[a] = lo;
+        d.hi[a] = hi;
+        d.step[a] = step;
+        d.inv[a] = n / (hi - lo);
+    }
+    for (int k = 0; k < s->planes; ++k) {
+        if (!std::isfinite(s->z[k]) || !std::isfinite(s->o[k][0]) || !std::isfinite(s->o[k][1]))
+            return RTX_E_BADARG;
+        d.z[k] = s->z[k];
+        d.o[k][0] = s->o[k][0];
+        d.o[k][1] = s->o[k][1];
+    }
+    d.c[0] = s->c[0];  // a NaN centre (a vignetted chief ray) is allowed: nothing is counted
+    d.c[1] = s->c[1];
+    d.counts = (unsigned long long*)counts;
+    return 0;
+}
+
+// the context's tally / extent accumulator, zeroed on the stream
+int spot_acc(rtx_ctx* ctx, SpotDev& d) {
+    if (!ctx->d_spot)
+        CK(cudaMalloc((void**)&ctx->d_spot, 5 * RTX_SPOT_MAX_PLANES * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(ctx->d_spot, 0, 5 * d.K * sizeof(unsigned long long), ctx->stream));
+    d.acc = ctx->d_spot;
+    return 0;
+}
+
+int spot_finish(rtx_ctx* ctx, const SpotDev& d, uint64_t* tally, double* extent) {
+    const int K = d.K;
+    unsigned long long h[5 * RTX_SPOT_MAX_PLANES];
+    CK(cudaMemcpyAsync(h, ctx->d_spot, 5 * K * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (tally)
+        for (int t = 0; t < 2 * K; ++t) tally[t] = h[t];
+    if (extent)
+        for (int t = 0; t < 3 * K; ++t) {
+            memcpy(extent + t, h + 2 * K + t, sizeof(double));
+            if (t % 3 == 2 && !d.radial) extent[t] = std::sqrt(extent[t]);  // the kernel kept r^2
+        }
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_spot(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, int dtype,
+                   int64_t N, const void* y0, const void* u0, int clip, const rtx_spot* spot,
+                   uint64_t* counts, uint64_t* tally, double* extent, unsigned flags) {
+    SpotDev sd;
+    int rc = spot_to_dev(spot, counts, extent, sd);
+    if (rc) return rc;
+    if (!ctx) return RTX_E_BADARG;
+    rc = check_table(surf, S);
+    if (rc) return rc;
+    if (N < 0 || !y0 || !u0) return RTX_E_BADARG;
+    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    rc = spot_acc(ctx, sd);
+    if (rc) return rc;
+    if (N > 0) {
+        CK(cudaEventRecord(ctx->k0, ctx->stream));
+        if (dtype == RTX_F64) {
+            EpiParams<double> p;
+            memset(&p, 0, sizeof(p));
+            p.spot = sd;
+            rc = launch_epi<double, EPI_SPOT>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
+        } else {
+            EpiParams<float> p;
+            memset(&p, 0, sizeof(p));
+            p.spot = sd;
+            rc = launch_epi<float, EPI_SPOT>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
+        }
+        if (rc) return rc;
+        CK(cudaEventRecord(ctx->k1, ctx->stream));
+        ctx->kernel_timed = true;
+    }
+    return spot_finish(ctx, sd, tally, extent);
+}
+
+int rtx_spot_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* inc,
+                  const rtx_spot* spot, uint64_t* counts, uint64_t* tally, double* extent) {
+    SpotDev sd;
+    int rc = spot_to_dev(spot, counts, extent, sd);
+    if (rc) return rc;
+    if (!ctx || N < 0 || !y || !inc) return RTX_E_BADARG;
+    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    rc = spot_acc(ctx, sd);
+    if (rc) return rc;
+    if (N > 0) {
+        long long blocks = (N + 255) / 256;
+        const long long cap = (long long)ctx->sm_count * 8;
+        if (blocks > cap) blocks = cap;
+        CK(cudaEventRecord(ctx->k0, ctx->stream));
+        if (dtype == RTX_F64)
+            spot_rows_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
+                sd, (const double*)y, (const double*)inc, N);
+        else
+            spot_rows_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
+                sd, (const float*)y, (const float*)inc, N);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(ctx->k1, ctx->stream));
+        ctx->kernel_timed = true;
+    }
+    return spot_finish(ctx, sd, tally, extent);
 }
 
 }  // extern "C"

@@ -21,6 +21,42 @@ OPD_DTYPE = np.dtype([("y0_ref", "<f8", (3,)), ("u0_ref", "<f8", (3,)), ("n0", "
                       ("n_after", "<f8"), ("M", "<f8", (9,)), ("d", "<f8", (3,)),
                       ("radius", "<f8"), ("infinite", "<i4"), ("reserved", "<i4")], align=True)
 
+# mirrors `struct rtx_spot` (include/rtx.h)
+SPOT_MAX_PLANES = 16
+SPOT_DTYPE = np.dtype([("planes", "<i4"), ("radial", "<i4"), ("nx", "<i8"), ("ny", "<i8"),
+                       ("range", "<f8", (2, 2)), ("c", "<f8", (2,)),
+                       ("z", "<f8", (SPOT_MAX_PLANES,)), ("o", "<f8", (SPOT_MAX_PLANES, 2))],
+                      align=True)
+
+
+def spot_spec(z, bins, range, center, radial=False, offsets=None):
+    """An rtx_spot record: defocus distances `z` (K,), `bins` (nx, ny) (radial:
+    nx or (nx,)), `range` ((x_lo, x_hi), (y_lo, y_hi)) (radial: (r_lo, r_hi)),
+    the chief intercept `center` (2,) and per-plane `offsets` (K, 2) or None.
+    The library checks the values (RtxError); more than 16 planes are passed
+    on as a count for it to refuse."""
+    z = np.atleast_1d(np.asarray(z, np.float64))
+    K = len(z)
+    rec = np.zeros(1, SPOT_DTYPE)
+    rec["planes"], rec["radial"] = K, int(bool(radial))
+    b = np.atleast_1d(np.asarray(bins, np.int64))
+    rec["nx"], rec["ny"] = (b[0], b[1]) if len(b) > 1 else (b[0], 1 if radial else b[0])
+    r = np.asarray(range, np.float64).reshape(-1, 2)
+    rec["range"][0, :len(r)] = r[:2]
+    rec["c"] = np.asarray(center, np.float64).reshape(2)
+    k = min(K, SPOT_MAX_PLANES)
+    rec["z"][0, :k] = z[:k]
+    if offsets is not None:
+        rec["o"][0, :k] = np.asarray(offsets, np.float64).reshape(K, 2)[:k]
+    return rec
+
+
+def spot_shape(spec):
+    """(K, nx, ny) of a 2-D record, (K, nx) of a radial one"""
+    s = spec[0]
+    K, nx = int(s["planes"]), int(s["nx"])
+    return (K, nx) if s["radial"] else (K, nx, int(s["ny"]))
+
 
 def _code(dtype):
     try:
@@ -546,6 +582,50 @@ class Engine:
         check(self.lib.rtx_trace_opd(
             self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
             int(bool(clip)), ptr(rec), A.ptr, P.ptr, self._flags(exact, False)))
+
+    @staticmethod
+    def _spot_outputs(spec, counts, extent):
+        """the record, host tally / extent buffers and the counts pointer;
+        ValueError for a counts array of another type or too small"""
+        spec = np.ascontiguousarray(spec, SPOT_DTYPE).reshape(1)
+        if counts is not None:
+            if np.dtype(counts.dtype) != np.uint64:
+                raise ValueError("counts must be uint64, got %s" % np.dtype(counts.dtype))
+            need = int(np.prod(spot_shape(spec), dtype=np.int64))
+            if 0 < need < 2**31 and counts.nbytes//8 < need:
+                raise ValueError("counts holds %d bins but the spec needs %d"
+                                 % (counts.nbytes//8, need))
+        K = max(int(spec[0]["planes"]), 1)
+        tally = np.zeros((K, 2), np.uint64)
+        ext = np.zeros((K, 3)) if extent else None
+        return spec, tally, ext, None if counts is None else counts.ptr
+
+    def trace_spot(self, table, y0, u0, spec, counts=None, N=None, clip=False, rot0=None,
+                   exact=False, extent=False):
+        """rtx_trace_spot: march the DEVICE launch rays to the last surface of
+        `table` and bin them at the planes of `spec` (spot_spec) into the
+        uint64 DeviceArray `counts` (added to; None: extent only) -- one
+        launch, nothing per ray is stored.  Returns (tally (K,2): binned,
+        non-finite; extent (K,3): max |q_x|, |q_y|, r, or None)."""
+        table = self._table(table)
+        N = y0.shape[0] if N is None else int(N)
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
+        spec, tally, ext, cp = self._spot_outputs(spec, counts, extent)
+        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
+        check(self.lib.rtx_trace_spot(
+            self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
+            int(bool(clip)), ptr(spec), cp, ptr(tally), ptr(ext), self._flags(exact, False)))
+        return tally, ext
+
+    def spot_rows(self, y, inc, spec, counts=None, N=None, extent=False):
+        """rtx_spot_rows: the binning of trace_spot on stored DEVICE rows
+        y, inc (N,3) (a trace's y[at], i[at]).  Same returns."""
+        N = y.shape[0] if N is None else int(N)
+        _check_operands(y.dtype, N, y=(y, 3), inc=(inc, 3))
+        spec, tally, ext, cp = self._spot_outputs(spec, counts, extent)
+        check(self.lib.rtx_spot_rows(self.ctx, _code(y.dtype), N, y.ptr, inc.ptr, ptr(spec), cp,
+                                     ptr(tally), ptr(ext)))
+        return tally, ext
 
     def ipc_export(self, darray):
         h = (C.c_ubyte*64)()

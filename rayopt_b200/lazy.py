@@ -321,16 +321,21 @@ class ResidentMixin:
 
 
     # ---- fused epilogues: the march itself reduces (no rows are stored or read)
-    def _guess_center(self, table, rot0, clip):
+    def _chief(self, table, rot0, clip):
         """(y_x, y_y, u_x, u_y) of the `ref` ray at the last surface of `table`
-        (a 1-ray trace through the small-bundle path), zeros if it dies"""
+        (a 1-ray trace through the small-bundle path); NaN if it dies"""
         eng, d = self._engine(), self._dev
         ref = 0 if self.ref is None else int(self.ref)
         y0 = eng.download_rays(d["y"].rows(0), [ref])
         u0 = eng.download_rays(d["u"].rows(0), [ref])
         Y, _, I, _ = eng.trace(table, y0, u0, clip=clip, rot0=rot0, keep_last=True,
                                exact=self.exact, want=("y", "i"))
-        c = np.r_[Y[0, 0, :2], I[0, 0, :2]/I[0, 0, 2]]
+        with np.errstate(all="ignore"):
+            return np.r_[Y[0, 0, :2], I[0, 0, :2]/I[0, 0, 2]].astype(np.float64)
+
+    def _guess_center(self, table, rot0, clip):
+        """the chief ray's (y_x, y_y, u_x, u_y), zeros if it dies"""
+        c = self._chief(table, rot0, clip)
         return c if np.all(np.isfinite(c)) else np.zeros(4)
 
     def reduce(self, at=-1, clip=False):
@@ -526,6 +531,54 @@ class ResidentMixin:
         ee = np.cumsum(bins)
         return dict(stats=st, x0=x0, y0=y0, dx=dx, center=center, xe=np.arange(ee.size)*dx,
                     ee=ee, of=of, mtf=tuple(mtf))
+
+
+    # ---- through-focus spot images (Analysis.spots, rayopt/analysis.py:250-283)
+    def spot_image(self, defocus=(0.,), bins=(256, 256), range=None, at=-1, radial=False,
+                   offsets=None, download=True):
+        """Spot images of the stored rows y[at], i[at] at the planes `defocus`
+        (rtx_spot_rows): the points ``y - y[ref] + z*tanarcsin(i) - offsets``
+        of Analysis.spots (analysis.py:266-280) binned as np.histogram2d
+        (radial: their radii as np.histogram) would bin them, exactly.  With
+        ``range=None`` an extent pass picks the symmetric range that holds
+        every finite point (spot.default_range).  A vignetted ref ray gives
+        a NaN centre and counts nothing.  Returns a dict: z, counts (K, nx,
+        ny) or (K, nx) uint64 (a DeviceArray when ``download=False``), edges,
+        range, tally (K, 2): rays binned, rays with a non-finite point."""
+        from .spot import spot_images
+        eng, d = self._engine(), self._dev
+        at = int(np.arange(self.length)[at])
+        ref = 0 if self.ref is None else int(self.ref)
+        c = eng.download_rays(d["y"].rows(at), [ref])[0, :2].astype(np.float64)
+
+        def part(spec, counts, extent):
+            return eng.spot_rows(d["y"].rows(at), d["i"].rows(at), spec, counts, N=self.nrays,
+                                 extent=extent)
+        return self._one_image(spot_images(eng, [(c, [part])], defocus, bins, range, radial,
+                                           offsets, download))
+
+    def spot_image_fused(self, defocus=(0.,), bins=(256, 256), range=None, at=-1, radial=False,
+                         offsets=None, download=True, clip=False):
+        """``spot_image`` of a march from the launch rays (row 0) to surface
+        `at` with the binning as its epilogue (rtx_trace_spot): no row is
+        stored or read.  The centre is the ref ray's, from a 1-ray trace."""
+        from .spot import spot_images
+        eng, d = self._engine(), self._dev
+        at = int(np.arange(self.length)[at])
+        table, _, rot0 = pack_system(self.system, self.l, 1, at + 1, n0=self.n[0])
+        c = self._chief(table, rot0, clip)[:2]
+
+        def part(spec, counts, extent):
+            return eng.trace_spot(table, d["y"].rows(0), d["u"].rows(0), spec, counts,
+                                  N=self.nrays, clip=clip, rot0=rot0, exact=self.exact,
+                                  extent=extent)
+        return self._one_image(spot_images(eng, [(c, [part])], defocus, bins, range, radial,
+                                           offsets, download))
+
+    @staticmethod
+    def _one_image(out):
+        out["counts"], out["tally"] = out["counts"][0], out["tally"][0]
+        return out
 
 
 class ResidentTrace(ResidentMixin):
