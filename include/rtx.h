@@ -660,6 +660,43 @@ int rtx_delaunay(rtx_ctx *ctx, int dtype, int64_t M, const void *pts, int64_t *T
  * a call only when the context keeps a smaller one) */
 int rtx_delaunay_bytes(rtx_ctx *ctx, int64_t M, size_t *bytes);
 
+/*
+ * The finite exit-pupil points of a per-ray OPD, compacted in HBM: what
+ * ResidentMixin.opd_rays and the filter of GeometricTrace.opd
+ * (rayopt/geometric_trace.py:125-135) compute on the host, bit for bit.
+ * A (N,) and P (N,3) are the DEVICE outputs of rtx_trace_opd (RTX_F64 only;
+ * RTX_F32 returns RTX_E_UNSUPPORTED).  With aref = A[ref], pref = P[ref], for
+ * each ray j, every operation separately rounded:
+ *   t = -(A[j] - aref)/k   (k = l/scale, the wavelength in lens units),
+ *   x = P[j].x - pref.x,  y = P[j].y - pref.y   (P[j].z plays no part).
+ * The rays with x, y and t all finite are written in increasing j to the
+ * DEVICE arrays pts (M,2) = (x, y) and vals (M,) = t; nothing is written at or
+ * after index M.  *M (host) receives the count, *h (host) max(|x|, |y|) over
+ * the kept rays (0 when M = 0).  A non-finite reference ray gives M = 0.
+ * The compaction is a prefix sum of the keep flags; the maximum an integer
+ * atomicMax on the bits of non-negative doubles: the same inputs give the
+ * same bits.  Workspace of 4 N bytes kept in the context; RTX_E_NOMEM before
+ * allocating it when it does not fit.  RTX_E_BADARG before any device work
+ * for a NULL ctx or pointer, N < 1 or N >= 2^31, ref outside [0, N), and k
+ * zero or not finite.  Synchronous (reads the 16 bytes of M and h);
+ * rtx_last_kernel_ms gives the device time of the call.
+ */
+int rtx_opd_points(rtx_ctx *ctx, int dtype, int64_t N, const void *A, const void *P,
+                   int64_t ref, double k, double *pts, double *vals, int64_t *M,
+                   double *h);
+
+/*
+ * Finite count, minimum and maximum of a DEVICE grid o (n,) (RTX_F64 only;
+ * RTX_F32 returns RTX_E_UNSUPPORTED): the PTP and the largest |o| Analysis.opds
+ * takes of the regridded OPD (rayopt/analysis.py:309-315).  NaN and +-inf
+ * are skipped; -0 counts below +0.  *count, *lo, *hi (host) receive the
+ * results; lo and hi are NaN when no value is finite.  Exact (integer
+ * atomics on order keys).  RTX_E_BADARG for a NULL ctx or pointer or n < 1.
+ * Synchronous; rtx_last_kernel_ms gives the device time of the call.
+ */
+int rtx_grid_range(rtx_ctx *ctx, int dtype, int64_t n, const void *o, int64_t *count,
+                   double *lo, double *hi);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,5 +14,6 @@ from . import elements  # noqa: F401
 from .lazy import LazyRows, ResidentMixin, ResidentTrace  # noqa: F401
 from ._lib import RtxError  # noqa: F401
 from .spot import spots  # noqa: F401
+from .opd import opds  # noqa: F401
 
 __version__ = "0.2.0"

@@ -80,6 +80,10 @@ SYMBOLS = {
     "rtx_selftest_predicates": (_i, [_vp, _i64, _vp, _vp]),
     "rtx_delaunay": (_i, [_vp, _i, _i64, _vp, C.POINTER(_i64), _vp, _vp, _vp]),
     "rtx_delaunay_bytes": (_i, [_vp, _i64, C.POINTER(_sz)]),
+    "rtx_opd_points": (_i, [_vp, _i, _i64, _vp, _vp, _i64, C.c_double, _vp, _vp,
+                            C.POINTER(_i64), C.POINTER(C.c_double)]),
+    "rtx_grid_range": (_i, [_vp, _i, _i64, _vp, C.POINTER(_i64), C.POINTER(C.c_double),
+                            C.POINTER(C.c_double)]),
 }
 
 _lib = None

@@ -122,6 +122,10 @@ struct rtx_ctx {
     // rtx_delaunay: slots, adjacency and point-location workspace
     void* d_dt = nullptr;
     size_t dt_cap = 0;
+    // rtx_opd_points: keep flags / ranks, block sums and max(|x|, |y|)
+    void* d_opd = nullptr;
+    size_t opd_cap = 0;
+    unsigned long long* d_range = nullptr;  // rtx_grid_range: count, min key, max key
 };
 
 namespace {
@@ -1005,6 +1009,8 @@ int rtx_free(rtx_ctx* ctx) {
     if (ctx->d_psf_red) cudaFree(ctx->d_psf_red);
     if (ctx->d_prof) cudaFree(ctx->d_prof);
     if (ctx->d_dt) cudaFree(ctx->d_dt);
+    if (ctx->d_opd) cudaFree(ctx->d_opd);
+    if (ctx->d_range) cudaFree(ctx->d_range);
     if (ctx->small_host) cudaFreeHost(ctx->small_host);
     if (ctx->small_dev) cudaFree(ctx->small_dev);
     if (ctx->t0) cudaEventDestroy(ctx->t0);
@@ -2404,6 +2410,103 @@ int rtx_delaunay(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, int64_t* T
     ctx->kernel_timed = true;
     CK(cudaStreamSynchronize(st));
     *T = nfin;
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- exit-pupil points and grid ranges of the OPD (rtx_psf.cuh) ------------
+extern "C" {
+
+int rtx_opd_points(rtx_ctx* ctx, int dtype, int64_t N, const void* A, const void* P, int64_t ref,
+                   double k, double* pts, double* vals, int64_t* M, double* h) {
+    // the prefix sum counts in int32
+    if (!ctx || !A || !P || !pts || !vals || !M || !h || N < 1 || N >= (1ll << 31) || ref < 0 ||
+        ref >= N || k == 0.0 || !std::isfinite(k))
+        return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    const int n = (int)N, nb = (n + dt::SCAN_THREADS - 1) / dt::SCAN_THREADS;
+    // [max bits | block sums and the total | keep flags, ranked in place]
+    const size_t bsum_off = 256, flag_off = bsum_off + ((size_t)(nb + 1) * 4 + 255) / 256 * 256;
+    const size_t need = flag_off + (size_t)n * 4;
+    if (need > ctx->opd_cap) {
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        if (need > free_b + ctx->opd_cap) return RTX_E_NOMEM;  // nothing allocated
+        if (ctx->d_opd) CK(cudaFree(ctx->d_opd));
+        ctx->d_opd = nullptr;
+        ctx->opd_cap = 0;
+        if (cudaMalloc(&ctx->d_opd, need) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->d_opd = nullptr;
+            return RTX_E_NOMEM;
+        }
+        ctx->opd_cap = need;
+    }
+    auto* hbits = (unsigned long long*)ctx->d_opd;
+    int* bsum = (int*)((char*)ctx->d_opd + bsum_off);
+    int* flag = (int*)((char*)ctx->d_opd + flag_off);
+    const double *a = (const double*)A, *p = (const double*)P;
+    cudaStream_t st = ctx->stream;
+    long long grid = (N + 255) / 256;
+    const long long cap = (long long)ctx->sm_count * 16;
+    if (grid > cap) grid = cap;
+    CK(cudaMemsetAsync(hbits, 0, 8, st));
+    CK(cudaEventRecord(ctx->k0, st));
+    opd_flag_kernel<<<(unsigned)grid, 256, 0, st>>>(a, p, N, ref, k, flag);
+    dt::scan_block_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum);
+    dt::scan_top_kernel<<<1, dt::SCAN_THREADS, 0, st>>>(bsum, nb);
+    // in place: each thread reads its own flag before the block scan and
+    // writes its rank after it
+    dt::scan_apply_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum, flag);
+    opd_scatter_kernel<<<(unsigned)grid, 256, 0, st>>>(a, p, N, ref, k, flag, pts, vals, hbits);
+    ctx->launches += 5;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, st));
+    ctx->kernel_timed = true;
+    int count = 0;
+    unsigned long long hb = 0;
+    CK(cudaMemcpyAsync(&count, bsum + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&hb, hbits, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    *M = count;
+    memcpy(h, &hb, 8);
+    return 0;
+}
+
+int rtx_grid_range(rtx_ctx* ctx, int dtype, int64_t n, const void* o, int64_t* count, double* lo,
+                   double* hi) {
+    if (!ctx || n < 1 || !o || !count || !lo || !hi) return RTX_E_BADARG;
+    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
+    if (dtype != RTX_F64) return RTX_E_BADARG;
+    CK(cudaSetDevice(ctx->device));
+    if (!ctx->d_range) CK(cudaMalloc((void**)&ctx->d_range, 3 * sizeof(unsigned long long)));
+    cudaStream_t st = ctx->stream;
+    long long grid = (n + 255) / 256;
+    const long long cap = (long long)ctx->sm_count * 8;
+    if (grid > cap) grid = cap;
+    CK(cudaMemsetAsync(ctx->d_range, 0, 3 * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(ctx->d_range + 1, 0xff, sizeof(unsigned long long), st));  // min key: ~0
+    CK(cudaEventRecord(ctx->k0, st));
+    grid_range_kernel<<<(unsigned)grid, 256, 0, st>>>((const double*)o, n, ctx->d_range);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->k1, st));
+    ctx->kernel_timed = true;
+    unsigned long long acc[3];
+    CK(cudaMemcpyAsync(acc, ctx->d_range, sizeof(acc), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    auto value = [](unsigned long long key) {  // order_key's inverse
+        const unsigned long long b = (key >> 63) ? key & ~0x8000000000000000ull : ~key;
+        double v;
+        memcpy(&v, &b, 8);
+        return v;
+    };
+    *count = (int64_t)acc[0];
+    *lo = acc[0] ? value(acc[1]) : NAN;
+    *hi = acc[0] ? value(acc[2]) : NAN;
     return 0;
 }
 

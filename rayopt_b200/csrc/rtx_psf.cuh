@@ -399,4 +399,93 @@ __global__ void __launch_bounds__(256) profile_combine_kernel(const double* __re
     }
 }
 
+// ---- exit-pupil points of the per-ray OPD (rtx_opd_points) ----------------
+//
+// Ray j's point and OPD relative to the reference ray, with numpy's separately
+// rounded operations (ResidentMixin.opd_rays): t = -(A[j] - A[ref])/k and
+// (x, y) = P[j].xy - P[ref].xy; the ray is kept when x, y and t are finite.
+// The kept rays are written in increasing j at the ranks an exclusive prefix
+// sum of the keep flags gives (dt::scan_*_kernel), so the compacted arrays are
+// those of numpy's boolean mask.
+struct OpdPoint {
+    double x, y, t;
+    bool keep;
+};
+
+__device__ __forceinline__ OpdPoint opd_point(const double* __restrict__ A, const double* __restrict__ P,
+                                              long long j, long long ref, double k) {
+    OpdPoint q;
+    q.t = __ddiv_rn(-__dsub_rn(A[j], A[ref]), k);
+    q.x = __dsub_rn(P[3 * j], P[3 * ref]);
+    q.y = __dsub_rn(P[3 * j + 1], P[3 * ref + 1]);
+    q.keep = isfinite(q.x) && isfinite(q.y) && isfinite(q.t);
+    return q;
+}
+
+__global__ void __launch_bounds__(256) opd_flag_kernel(const double* __restrict__ A,
+                                                       const double* __restrict__ P, long long N,
+                                                       long long ref, double k, int* __restrict__ flag) {
+    for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j < N;
+         j += (long long)gridDim.x * blockDim.x)
+        flag[j] = opd_point(A, P, j, ref, k).keep ? 1 : 0;
+}
+
+// the kept rays to their ranks; hbits receives max(|x|, |y|) of them as the
+// bits of a non-negative double, whose integer order is the numeric order
+__global__ void __launch_bounds__(256) opd_scatter_kernel(
+    const double* __restrict__ A, const double* __restrict__ P, long long N, long long ref, double k,
+    const int* __restrict__ rank, double* __restrict__ pts, double* __restrict__ vals,
+    unsigned long long* __restrict__ hbits) {
+    unsigned long long m = 0;
+    for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j < N;
+         j += (long long)gridDim.x * blockDim.x) {
+        const OpdPoint q = opd_point(A, P, j, ref, k);
+        if (!q.keep) continue;
+        const long long r = rank[j];
+        pts[2 * r] = q.x;
+        pts[2 * r + 1] = q.y;
+        vals[r] = q.t;
+        const unsigned long long bx = (unsigned long long)__double_as_longlong(fabs(q.x));
+        const unsigned long long by = (unsigned long long)__double_as_longlong(fabs(q.y));
+        m = max(m, max(bx, by));
+    }
+    for (int off = 16; off; off >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, off));
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(hbits, m);
+}
+
+// ---- finite count, min and max of a grid (rtx_grid_range) ------------------
+//
+// Integer atomics on order keys (the sign bit flipped for non-negative values,
+// every bit for negative ones): the unsigned order of the keys is the numeric
+// order with -0 < +0, so the result is exact and independent of the schedule.
+// acc = {count, min key, max key}, initialised to {0, ~0, 0}.
+__device__ __forceinline__ unsigned long long order_key(double v) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+    return (b >> 63) ? ~b : b | 0x8000000000000000ull;
+}
+
+__global__ void __launch_bounds__(256) grid_range_kernel(const double* __restrict__ o, long long n,
+                                                         unsigned long long* __restrict__ acc) {
+    unsigned long long c = 0, lo = ~0ull, hi = 0;
+    for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < n;
+         k += (long long)gridDim.x * blockDim.x) {
+        const double v = o[k];
+        if (!isfinite(v)) continue;
+        const unsigned long long key = order_key(v);
+        ++c;
+        lo = min(lo, key);
+        hi = max(hi, key);
+    }
+    for (int off = 16; off; off >>= 1) {
+        c += __shfl_down_sync(0xffffffffu, c, off);
+        lo = min(lo, __shfl_down_sync(0xffffffffu, lo, off));
+        hi = max(hi, __shfl_down_sync(0xffffffffu, hi, off));
+    }
+    if ((threadIdx.x & 31) == 0 && c) {
+        atomicAdd(acc, c);
+        atomicMin(acc + 1, lo);
+        atomicMax(acc + 2, hi);
+    }
+}
+
 }  // namespace rtx

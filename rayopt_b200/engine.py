@@ -791,22 +791,24 @@ class Engine:
         fill_value=nan) on the grid node (i, j) = (gh[i], gh[j]), with the
         triangulation `tri` of `points`: scipy.spatial.Delaunay on the host,
         or a DeviceTriangulation (``delaunay``), whose arrays are used in place;
-        `points` may be a DeviceArray, used in place too.
+        `points` and `values` may be DeviceArrays, used in place too.
         Returns the (n, n) values -- numpy, or a DeviceArray when not
         `download` -- and with `winner` also the covering simplex per node
         (numpy int32, -1 where none covers it, like find_simplex)."""
         dev_points = isinstance(points, DeviceArray)
+        dev_values = isinstance(values, DeviceArray)
         if not dev_points:
             points = np.ascontiguousarray(points, np.float64)
-        values = np.ascontiguousarray(values, np.float64)
+        if not dev_values:
+            values = np.ascontiguousarray(values, np.float64)
         gh = np.ascontiguousarray(gh, np.float64)
         if len(points.shape) != 2 or points.shape[1] != 2 or values.shape != points.shape[:1] \
-                or np.dtype(points.dtype) != np.float64:
+                or np.dtype(points.dtype) != np.float64 or np.dtype(values.dtype) != np.float64:
             raise ValueError("points must be (M, 2) FP64 and values (M,)")
         if gh.shape != (int(n),):
             raise ValueError("gh must be the (n,) grid axis")
         n = int(n)
-        ins = [self.to_device(a) for a in (values, gh)]
+        ins = [values if dev_values else self.to_device(values), self.to_device(gh)]
         if not dev_points:
             ins.append(self.to_device(points))
         pts_ptr = points.ptr if dev_points else ins[-1].ptr
@@ -835,9 +837,44 @@ class Engine:
             else:
                 self.sync()
         finally:
-            for a in ins:
+            for a in ins[1:] if dev_values else ins:
                 a.free()
         return (out, w) if winner else out
+
+    def opd_points(self, A, P, ref, k):
+        """rtx_opd_points: the finite exit-pupil points of rtx_trace_opd's
+        DEVICE outputs A (N,), P (N,3) relative to ray `ref`, compacted in
+        ray order, with t = -(A - A[ref])/k, k = l/scale.  Returns (pts
+        DeviceArray (M, 2), vals DeviceArray (M,), M, h = max |x|, |y|); the
+        arrays hold room for N rays, free them when done."""
+        N = int(A.shape[0])
+        if A.dtype != np.float64 or P.dtype != np.float64 or P.shape[:1] != (N,) or \
+                len(P.shape) != 2 or P.shape[1] != 3:
+            raise ValueError("A must be (N,) and P (N, 3) FP64 device arrays")
+        pts, vals = self.empty((max(N, 1), 2)), self.empty((max(N, 1),))
+        M, h = C.c_int64(), C.c_double()
+        try:
+            check(self.lib.rtx_opd_points(self.ctx, RTX_F64, N, A.ptr, P.ptr, int(ref), float(k),
+                                          pts.ptr, vals.ptr, C.byref(M), C.byref(h)))
+        except Exception:
+            pts.free()
+            vals.free()
+            raise
+        M = int(M.value)
+        for a in (pts, vals):               # M rows of the N-ray allocation
+            a.shape = (M,) + a.shape[1:]
+            a.nbytes = M*a.nbytes//max(N, 1)
+        return pts, vals, M, float(h.value)
+
+    def grid_range(self, o):
+        """rtx_grid_range of a DEVICE FP64 array: (finite count, min, max)
+        over its finite values, NaN min and max when there are none"""
+        if o.dtype != np.float64:
+            raise ValueError("o must be an FP64 device array")
+        count, lo, hi = C.c_int64(), C.c_double(), C.c_double()
+        check(self.lib.rtx_grid_range(self.ctx, RTX_F64, int(np.prod(o.shape)), o.ptr,
+                                      C.byref(count), C.byref(lo), C.byref(hi)))
+        return int(count.value), float(lo.value), float(hi.value)
 
     def selftest_predicates(self, quads):
         """(n, 2) int: the device's exact orient2d(a, b, c) and incircle(a, b,

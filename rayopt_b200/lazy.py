@@ -23,6 +23,101 @@ from .surface_table import pack_system
 PINNED_ROW_BYTES = 1 << 20
 
 
+def opd_spec(system, track, origins, after, image, n0, n_after, y0_ref, u0_ref, y_img_ref,
+             radius=None):
+    """The `rtx_opd` record of GeometricTrace.opd (rayopt/geometric_trace.py:
+    101-131) for surfaces `after` and `image` (indices >= 0): the default
+    reference-sphere radius (:110-114, the image pupil's distance, or the
+    track between the surfaces for a telecentric pupil), the frame change
+    between the surfaces (their rotations and origins) and the reference
+    ray's launch ray (y0_ref, u0_ref) and image intercept y_img_ref."""
+    s = system
+    if radius is None:                                  # :110-114
+        if s.image.pupil.telecentric:
+            radius = track[image] - track[after]
+        else:
+            radius = -s.image.pupil.distance
+    ea, ei = s[after], s[image]
+    eye = np.eye(3)
+    Ra = np.asarray(ea.rot_normal, float) if getattr(ea, "rotated", False) else eye
+    Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else eye
+    return dict(y0_ref=y0_ref, u0_ref=u0_ref, n0=n0, n_after=n_after, M=Ra @ Ri.T,
+                d=(origins[after] - origins[image]) @ Ri.T - y_img_ref,
+                radius=radius, infinite=not s.object.finite)
+
+
+def check_triangulation(triangulation):
+    if triangulation not in ("host", "device"):
+        raise ValueError("triangulation must be 'host' or 'device', got %r" % (triangulation,))
+
+
+def regrid(eng, pts, vals, M, h, n, download, triangulation):
+    """GeometricTrace.opd's regridding (rayopt/geometric_trace.py:136-143) of
+    the M compacted exit-pupil points `pts`, `vals` (Engine.opd_points; freed
+    here) on the (n, n) grid of half-width h: Delaunay on the host (the
+    points downloaded) or on the device, then rtx_grid_linear.  Returns
+    (xs, ys, o) with o numpy, or a DeviceArray when not `download`.
+    ValueError when no ray made it through."""
+    try:
+        if not M:
+            raise ValueError("no rays made it through")
+        xs, ys = np.mgrid[-1:1:1j*n, -1:1:1j*n]*h
+        if triangulation == "host":
+            from scipy.spatial import Delaunay
+            p, v = pts.download(), vals.download()
+            return xs, ys, eng.grid_linear(p, v, Delaunay(p), n, xs[:, 0].copy(),
+                                           download=download)
+        tri = eng.delaunay(pts)
+        try:
+            return xs, ys, eng.grid_linear(pts, vals, tri, n, xs[:, 0].copy(), download=download)
+        finally:
+            tri.free()
+    finally:
+        pts.free()
+        vals.free()
+
+
+def psf_of_grid(eng, xs, o, pad, wl, radius):
+    """GeometricTrace.psf (rayopt/geometric_trace.py:150-161) of the
+    regridded OPD `o` (DEVICE (n, n), freed here) on the grid `xs`: rtx_psf
+    and the frequency axes for the wavelength wl = l/scale in lens units and
+    the sphere's radius.  Returns (p, q, psf DeviceArray, stats)."""
+    try:
+        out, raw = eng.psf(o, pad)
+    finally:
+        o.free()
+    nx = pad*xs.shape[0]
+    dx = xs[1, 0] - xs[0, 0]
+    k = 1/wl
+    f = np.fft.fftfreq(nx, dx*k/radius)
+    p, q = np.broadcast_arrays(f[:, None], f)
+    return p, q, out, eng.psf_stats(raw, f)
+
+
+def psf_profiles(eng, p, out, st):
+    """The encircled energy and MTF Analysis.opds (rayopt/analysis.py:
+    319-346) takes of the DEVICE PSF `out` (freed here) on the axis `p`,
+    with its device stats `st` (ResidentMixin.psf_profiles)"""
+    try:
+        x0, y0 = st["cp"], st["cq"]
+        xs = np.fft.fftshift(p[:, 0])
+        dx = (xs[1] - x0) - (xs[0] - x0)
+        nx, ny = out.shape
+        center = (nx/2 + x0/dx, ny/2 + y0/dx)
+        bins, lsf0, lsf1 = eng.psf_profiles(out, center)
+    finally:
+        out.free()
+    size = nx*ny
+    mtf = []
+    for lsf in (lsf0, lsf1):
+        ot = np.fft.ifft(lsf*size**.5)
+        mtf.append(np.absolute(ot[:ot.size//2]))
+    of = np.fft.fftfreq(lsf0.size, dx)[:lsf0.size//2]
+    ee = np.cumsum(bins)
+    return dict(stats=st, x0=x0, y0=y0, dx=dx, center=center, xe=np.arange(ee.size)*dx,
+                ee=ee, of=of, mtf=tuple(mtf))
+
+
 class LazyRows:
     """numpy-like view of a device array (rows, ld, k...) restricted to the
     first `n` columns.  Indexing with a leading integer (or a slice of rows)
@@ -366,6 +461,23 @@ class ResidentMixin:
         self.system[at].distance += shift
         return shift
 
+    def _trace_opd(self, radius, after, image):
+        """rtx_trace_opd from row 0 to surface `after`: DEVICE A (N,), P (N,3)
+        (free them when done).  Needs a propagated trace (the sphere is
+        centred on ``y[image, ref]``)."""
+        eng, s, d = self._engine(), self.system, self._dev
+        after, image = range(self.length)[after], range(self.length)[image]
+        ref = int(self.ref)
+        spec = opd_spec(s, self.track, self.origins, after, image, self.n[0], self.n[after],
+                        eng.download_rays(d["y"].rows(0), [ref])[0],
+                        eng.download_rays(d["u"].rows(0), [ref])[0],
+                        eng.download_rays(d["y"].rows(image), [ref])[0], radius)
+        table, _, rot0 = pack_system(s, self.l, 1, after + 1, n0=self.n[0])
+        A, P = eng.empty((self.nrays,)), eng.empty((self.nrays, 3))
+        eng.trace_opd(table, d["y"].rows(0), d["u"].rows(0), spec, A, P, N=self.nrays,
+                      clip=getattr(self, "_last_clip", False), rot0=rot0, exact=self.exact)
+        return A, P
+
     def opd_rays(self, radius=None, after=-2, image=-1):
         """per-ray part of GeometricTrace.opd (rayopt/geometric_trace.py:
         101-131) as the epilogue of a march from row 0 to surface `after`
@@ -373,32 +485,12 @@ class ResidentMixin:
         Returns (x, y, t): exit-pupil coordinates and the OPD in waves -- what
         ``opd(resample=False)`` returns in the reference.  Needs a propagated
         trace (the sphere is centred on ``y[image, ref]``)."""
-        eng, s, d = self._engine(), self.system, self._dev
-        after, image = range(self.length)[after], range(self.length)[image]
-        ref = int(self.ref)
-        if radius is None:                                  # :110-114
-            if s.image.pupil.telecentric:
-                radius = self.track[image] - self.track[after]
-            else:
-                radius = -s.image.pupil.distance
-        ea, ei = s[after], s[image]
-        eye = np.eye(3)
-        Ra = np.asarray(ea.rot_normal, float) if getattr(ea, "rotated", False) else eye
-        Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else eye
-        y_img_ref = eng.download_rays(d["y"].rows(image), [ref])[0]
-        spec = dict(y0_ref=eng.download_rays(d["y"].rows(0), [ref])[0],
-                    u0_ref=eng.download_rays(d["u"].rows(0), [ref])[0],
-                    n0=self.n[0], n_after=self.n[after], M=Ra @ Ri.T,
-                    d=(self.origins[after] - self.origins[image]) @ Ri.T - y_img_ref,
-                    radius=radius, infinite=not s.object.finite)
-        table, _, rot0 = pack_system(s, self.l, 1, after + 1, n0=self.n[0])
-        A, P = eng.empty((self.nrays,)), eng.empty((self.nrays, 3))
-        eng.trace_opd(table, d["y"].rows(0), d["u"].rows(0), spec, A, P, N=self.nrays,
-                      clip=getattr(self, "_last_clip", False), rot0=rot0, exact=self.exact)
+        A, P = self._trace_opd(radius, after, image)
         a, p = A.download(), P.download()
         A.free()
         P.free()
-        t = -(a - a[ref])/(self.l/s.scale)                  # :125-126
+        ref = int(self.ref)
+        t = -(a - a[ref])/(self.l/self.system.scale)        # :125-126
         p -= p[ref]                                         # :131
         return p[:, 0], p[:, 1], t
 
@@ -421,37 +513,21 @@ class ResidentMixin:
 
     # ---- diffraction PSF with the regridding and the FFT on the device
     def _opd_grid(self, radius, after, image, resample, download, triangulation="host"):
-        """opd's regridding on the device: the finite exit-pupil points are
-        triangulated on the host (scipy.spatial.Delaunay, griddata's own
-        options) or, with ``triangulation="device"``, uploaded once and
-        triangulated in HBM (rtx_delaunay); rtx_grid_linear interpolates on
-        the reference's grid"""
-        if triangulation not in ("host", "device"):
-            raise ValueError("triangulation must be 'host' or 'device', got %r" % (triangulation,))
-        x, y, t = self.opd_rays(radius, after, image)
-        ok = np.isfinite(x) & np.isfinite(y) & np.isfinite(t)
-        x, y, t = x[ok], y[ok], t[ok]
-        if not t.size:
-            raise ValueError("no rays made it through")
-        n = int(resample*self.nrays**.5)
-        h = np.fabs((x, y)).max()
-        xs, ys = np.mgrid[-1:1:1j*n, -1:1:1j*n]*h
-        pts = np.stack([x, y], axis=-1)
+        """opd's regridding on the device: the per-ray OPD (rtx_trace_opd)
+        and its finite exit-pupil points (rtx_opd_points) stay in HBM; they
+        are triangulated on the host (scipy.spatial.Delaunay of the M
+        downloaded points, griddata's own options) or, with
+        ``triangulation="device"``, in HBM (rtx_delaunay); rtx_grid_linear
+        interpolates on the reference's grid"""
+        check_triangulation(triangulation)
         eng = self._engine()
-        if triangulation == "host":
-            from scipy.spatial import Delaunay
-            return xs, ys, eng.grid_linear(pts, t, Delaunay(pts), n, xs[:, 0].copy(),
-                                           download=download)
-        dpts = eng.to_device(pts)
+        A, P = self._trace_opd(radius, after, image)
         try:
-            tri = eng.delaunay(dpts)
-            try:
-                o = eng.grid_linear(dpts, t, tri, n, xs[:, 0].copy(), download=download)
-            finally:
-                tri.free()
+            pts = eng.opd_points(A, P, int(self.ref), self.l/self.system.scale)
         finally:
-            dpts.free()
-        return xs, ys, o
+            A.free()
+            P.free()
+        return regrid(eng, *pts, int(resample*self.nrays**.5), download, triangulation)
 
     def opd_device(self, radius=None, after=-2, image=-1, resample=4, triangulation="host"):
         """``opd`` (rayopt/geometric_trace.py:101-144) with the regridding on
@@ -483,16 +559,7 @@ class ResidentMixin:
             raise TypeError("unexpected arguments %s" % sorted(kwargs))
         xs, ys, o = self._opd_grid(radius, after, image, resample, download=False,
                                    triangulation=triangulation)
-        try:
-            out, raw = eng.psf(o, pad)
-        finally:
-            o.free()
-        nx = pad*xs.shape[0]
-        dx = xs[1, 0] - xs[0, 0]
-        k = 1/(self.l/self.system.scale)
-        f = np.fft.fftfreq(nx, dx*k/radius)
-        p, q = np.broadcast_arrays(f[:, None], f)
-        self.psf_stats = eng.psf_stats(raw, f)
+        p, q, out, self.psf_stats = psf_of_grid(eng, xs, o, pad, self.l/self.system.scale, radius)
         if download:
             psf = out.download()
             out.free()
@@ -512,26 +579,7 @@ class ResidentMixin:
         in ``psf_device``."""
         p, q, out = self.psf_device(pad, resample, download=False, triangulation=triangulation,
                                     **kwargs)
-        try:
-            st = self.psf_stats
-            x0, y0 = st["cp"], st["cq"]
-            xs = np.fft.fftshift(p[:, 0])
-            dx = (xs[1] - x0) - (xs[0] - x0)
-            nx, ny = out.shape
-            center = (nx/2 + x0/dx, ny/2 + y0/dx)
-            bins, lsf0, lsf1 = self._engine().psf_profiles(out, center)
-        finally:
-            out.free()
-        size = nx*ny
-        mtf = []
-        for lsf in (lsf0, lsf1):
-            ot = np.fft.ifft(lsf*size**.5)
-            mtf.append(np.absolute(ot[:ot.size//2]))
-        of = np.fft.fftfreq(lsf0.size, dx)[:lsf0.size//2]
-        ee = np.cumsum(bins)
-        return dict(stats=st, x0=x0, y0=y0, dx=dx, center=center, xe=np.arange(ee.size)*dx,
-                    ee=ee, of=of, mtf=tuple(mtf))
-
+        return psf_profiles(self._engine(), p, out, self.psf_stats)
 
     # ---- through-focus spot images (Analysis.spots, rayopt/analysis.py:250-283)
     def spot_image(self, defocus=(0.,), bins=(256, 256), range=None, at=-1, radial=False,
