@@ -94,7 +94,8 @@ extern "C" {
 #define RTX_OK              0
 #define RTX_E_BADARG       -1
 #define RTX_E_UNSUPPORTED  -2
-#define RTX_E_NOMEM        -3
+#define RTX_E_NOMEM        -3 /* also: a buffer the context keeps across calls could
+                                 not grow; the old one is kept and nothing is freed */
 
 /*
  * One traced surface for one wavelength: everything System.propagate

@@ -68,6 +68,28 @@ struct Tuning {
     int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
 };
 
+// A device buffer of the context kept across calls: it grows (reserve) and
+// never shrinks.
+struct Workspace {
+    void* p = nullptr;
+    size_t cap = 0;
+};
+
+// the context's workspaces (rtx_ctx::ws)
+enum {
+    WS_MOMENTS,  // rtx_moments, rtx_focus_moments: the 8 sums
+    WS_EPI,      // rtx_trace_reduce: the RTX_NMOMENTS sums
+    WS_SPOT,     // rtx_trace_spot / rtx_spot_rows: tallies, extents
+    WS_AIM,      // rtx_aim_plan: per-block counts, then the offsets of the kept rays
+    WS_WINNER,   // rtx_grid_linear: claim grid when the caller wants no winner output
+    WS_PSF_RED,  // rtx_psf: partial sums, the finite count and the stats
+    WS_PROF,     // rtx_psf_profiles: per-block partial rows, their sum and the pixel flag
+    WS_DT,       // rtx_delaunay: slots, adjacency and point-location workspace
+    WS_OPD,      // rtx_opd_points: keep flags / ranks, block sums and max(|x|, |y|)
+    WS_RANGE,    // rtx_grid_range: count, min key, max key
+    WS_COUNT
+};
+
 }  // namespace
 
 struct rtx_ctx {
@@ -82,14 +104,10 @@ struct rtx_ctx {
     int next_slot = 0;
     size_t slot_bytes = 0;
     ChunkBuf chunk[2];
-    double* d_moments = nullptr;
-    double* d_epi = nullptr;  // rtx_trace_reduce
-    unsigned long long* d_spot = nullptr;  // rtx_trace_spot / rtx_spot_rows: tallies, extents
+    Workspace ws[WS_COUNT];
     // cached plan of the ray generator (rtx_aim_plan / rtx_aim_rays)
     std::vector<unsigned char> aim_key;
     std::vector<long long> aim_offsets;  // per block; empty: nothing is rejected
-    long long* d_aim_offsets = nullptr;
-    size_t d_aim_cap = 0;
     long long aim_total = 0, aim_M = 0;
     // small-bundle latency path (ray aiming: hundreds of 1-3 ray traces)
     void* small_host = nullptr;  // pinned: [y0|u0] in, [Y|U|I|T] out
@@ -106,26 +124,12 @@ struct rtx_ctx {
     // rtx_numa_bind: what to restore
     bool numa_bound = false;
     cpu_set_t saved_affinity;
-    // rtx_grid_linear: claim grid when the caller wants no winner output
-    int* d_winner = nullptr;
-    size_t winner_cap = 0;
     // rtx_psf: the cuFFT plan of the last (nx, ny) and its work area
     cufftHandle fft_plan = 0;
     bool fft_planned = false;
     long long fft_nx = 0, fft_ny = 0;
     void* fft_work = nullptr;
     size_t fft_work_bytes = 0;
-    double* d_psf_red = nullptr;  // partial sums, the finite count and the stats
-    // rtx_psf_profiles: per-block partial rows, their sum and the pixel flag
-    double* d_prof = nullptr;
-    size_t prof_cap = 0;
-    // rtx_delaunay: slots, adjacency and point-location workspace
-    void* d_dt = nullptr;
-    size_t dt_cap = 0;
-    // rtx_opd_points: keep flags / ranks, block sums and max(|x|, |y|)
-    void* d_opd = nullptr;
-    size_t opd_cap = 0;
-    unsigned long long* d_range = nullptr;  // rtx_grid_range: count, min key, max key
 };
 
 namespace {
@@ -401,10 +405,90 @@ int check_table(const rtx_surface* surf, int S) {
     return 0;
 }
 
-bool valid_keep_dtype(int keep, int dtype) {
-    return (keep == RTX_KEEP_ALL || keep == RTX_KEEP_LAST) &&
-           (dtype == RTX_F64 || dtype == RTX_F32);
+// the table and the launch rays of a march
+int check_march(const rtx_surface* surf, int S, long long N, const void* y0, const void* u0) {
+    int rc = check_table(surf, S);
+    if (rc) return rc;
+    return N < 0 || !y0 || !u0 ? RTX_E_BADARG : 0;
 }
+
+bool valid_keep(int keep) { return keep == RTX_KEEP_ALL || keep == RTX_KEEP_LAST; }
+
+// f(double()) or f(float()) by the element type code; RTX_E_BADARG for any other
+template <typename F>
+int dispatch(int dtype, F&& f) {
+    if (dtype == RTX_F64) return f(double());
+    if (dtype == RTX_F32) return f(float());
+    return RTX_E_BADARG;
+}
+
+// the element type check of the calls that compute in FP64 only
+int fp64_only(int dtype) {
+    if (dtype == RTX_F64) return 0;
+    return dtype == RTX_F32 ? RTX_E_UNSUPPORTED : RTX_E_BADARG;
+}
+
+// Runs `region` (the device work of one call) between the context's events k0
+// and k1.  rtx_last_kernel_ms reports that span only when the region succeeded.
+template <typename F>
+int timed(rtx_ctx* ctx, F&& region) {
+    ctx->kernel_timed = false;
+    CK(cudaEventRecord(ctx->k0, ctx->stream));
+    int rc = region();
+    if (rc) return rc;
+    CK(cudaEventRecord(ctx->k1, ctx->stream));
+    ctx->kernel_timed = true;
+    return 0;
+}
+
+// blocks of a grid-stride launch: at least one, at most per_sm per SM.  The
+// reductions sum their block partials in an order that depends on the grid.
+unsigned cap_grid(const rtx_ctx* ctx, long long nblocks, int per_sm) {
+    return (unsigned)std::clamp(nblocks, 1ll, (long long)ctx->sm_count * per_sm);
+}
+
+// Makes `ws` hold at least `bytes`.  RTX_E_NOMEM, with the old buffer kept,
+// when they do not fit in free device memory plus that buffer.
+int reserve(Workspace& ws, size_t bytes) {
+    if (bytes <= ws.cap) return 0;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes > free_b + ws.cap) return RTX_E_NOMEM;  // nothing freed
+    if (ws.p) CK(cudaFree(ws.p));
+    ws = Workspace();
+    if (cudaMalloc(&ws.p, bytes) != cudaSuccess) {
+        cudaGetLastError();  // (clear it)
+        ws = Workspace();
+        return RTX_E_NOMEM;
+    }
+    ws.cap = bytes;
+    return 0;
+}
+
+// owner of one temporary cudaMalloc allocation, freed on every return path
+class DeviceBuf {
+  public:
+    DeviceBuf() = default;
+    DeviceBuf(DeviceBuf&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+    DeviceBuf(const DeviceBuf&) = delete;
+    DeviceBuf& operator=(const DeviceBuf&) = delete;
+    ~DeviceBuf() {
+        if (p_) cudaFree(p_);
+    }
+    cudaError_t alloc(size_t bytes) {
+        cudaError_t e = cudaMalloc(&p_, bytes);
+        if (e != cudaSuccess) p_ = nullptr;
+        return e;
+    }
+    void* get() const { return p_; }
+    template <typename T>
+    T* as() const {
+        return static_cast<T*>(p_);
+    }
+
+  private:
+    void* p_ = nullptr;
+};
 
 struct PeerDst {
     int n = 0;
@@ -948,7 +1032,6 @@ int rtx_init(int device, rtx_ctx** out) {
         CK(cudaEventCreate(&ctx->t1));
         CK(cudaEventCreate(&ctx->k0));
         CK(cudaEventCreate(&ctx->k1));
-        CK(cudaMalloc((void**)&ctx->d_moments, 8 * sizeof(double)));
         return 0;
     };
     if (int rc = setup()) {
@@ -1000,17 +1083,9 @@ int rtx_free(rtx_ctx* ctx) {
     }
     free_chunk(ctx->chunk[0]);
     free_chunk(ctx->chunk[1]);
-    if (ctx->d_moments) cudaFree(ctx->d_moments);
-    if (ctx->d_epi) cudaFree(ctx->d_epi);
-    if (ctx->d_spot) cudaFree(ctx->d_spot);
-    if (ctx->d_aim_offsets) cudaFree(ctx->d_aim_offsets);
-    if (ctx->d_winner) cudaFree(ctx->d_winner);
+    for (Workspace& w : ctx->ws)
+        if (w.p) cudaFree(w.p);
     release_fft_plan(ctx);
-    if (ctx->d_psf_red) cudaFree(ctx->d_psf_red);
-    if (ctx->d_prof) cudaFree(ctx->d_prof);
-    if (ctx->d_dt) cudaFree(ctx->d_dt);
-    if (ctx->d_opd) cudaFree(ctx->d_opd);
-    if (ctx->d_range) cudaFree(ctx->d_range);
     if (ctx->small_host) cudaFreeHost(ctx->small_host);
     if (ctx->small_dev) cudaFree(ctx->small_dev);
     if (ctx->t0) cudaEventDestroy(ctx->t0);
@@ -1198,24 +1273,17 @@ int rtx_trace(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, 
               int64_t N, const void* y0, const void* u0, int clip, int keep, int64_t ld, void* Y,
               void* U, void* I, void* T, unsigned flags) {
     if (!ctx) return RTX_E_BADARG;
-    int rc = check_table(surf, S);
+    int rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || ld < N || !y0 || !u0) return RTX_E_BADARG;
-    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    if (dtype == RTX_F64) {
-        Launch<double> L(surf, S, rot0, clip, keep, ld, flags);
-        rc = trace_registered(ctx, L, surf, N, y0, u0, Y, U, I, T);
-    } else {
-        Launch<float> L(surf, S, rot0, clip, keep, ld, flags);
-        rc = trace_registered(ctx, L, surf, N, y0, u0, Y, U, I, T);
-    }
-    if (rc) return rc;
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
-    return 0;
+    if (ld < N || !valid_keep(keep)) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        if (N == 0) return 0;
+        CK(cudaSetDevice(ctx->device));
+        return timed(ctx, [&] {
+            Launch<decltype(t)> L(surf, S, rot0, clip, keep, ld, flags);
+            return trace_registered(ctx, L, surf, N, y0, u0, Y, U, I, T);
+        });
+    });
 }
 
 }  // extern "C"
@@ -1243,23 +1311,19 @@ int rtx_trace_batch(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, int S,
                     const void* const* u0, int clip, int keep, int64_t ld, void* const* Y,
                     void* const* U, void* const* I, void* const* T, unsigned flags) {
     if (!ctx || nb < 1 || nb > RTX_MAX_BATCH || !surf || !N || !y0 || !u0) return RTX_E_BADARG;
-    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
-    for (int b = 0; b < nb; ++b) {
-        int rc = check_table(surf[b], S);
-        if (rc) return rc;
-        if (N[b] < 1 || ld < N[b] || !y0[b] || !u0[b]) return RTX_E_BADARG;
-    }
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    int rc = dtype == RTX_F64
-                 ? trace_batch<double>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I,
-                                       T, flags)
-                 : trace_batch<float>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, ld, Y, U, I, T,
-                                      flags);
-    if (rc) return rc;
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
-    return 0;
+    if (!valid_keep(keep)) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        for (int b = 0; b < nb; ++b) {
+            int rc = check_table(surf[b], S);
+            if (rc) return rc;
+            if (N[b] < 1 || ld < N[b] || !y0[b] || !u0[b]) return RTX_E_BADARG;
+        }
+        CK(cudaSetDevice(ctx->device));
+        return timed(ctx, [&] {
+            return trace_batch<decltype(t)>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, ld, Y,
+                                            U, I, T, flags);
+        });
+    });
 }
 
 }  // extern "C"
@@ -1364,32 +1428,32 @@ int rtx_trace_batch_host(rtx_ctx* ctx, int nb, const rtx_surface* const* surf, i
                          const void* const* u0, int clip, int keep, void* const* Y,
                          void* const* U, void* const* I, void* const* T, unsigned flags) {
     if (!ctx || nb < 1 || !surf || !N || !y0 || !u0) return RTX_E_BADARG;
-    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
-    for (int b = 0; b < nb; ++b) {
-        int rc = check_table(surf[b], S);
-        if (rc) return rc;
-        if (N[b] < 0 || (N[b] > 0 && (!y0[b] || !u0[b]))) return RTX_E_BADARG;
-    }
-    CK(cudaSetDevice(ctx->device));
-    return dtype == RTX_F64 ? trace_batch_host<double>(ctx, nb, surf, S, rot0, N, y0, u0, clip,
-                                                       keep, Y, U, I, T, flags)
-                            : trace_batch_host<float>(ctx, nb, surf, S, rot0, N, y0, u0, clip,
-                                                      keep, Y, U, I, T, flags);
+    if (!valid_keep(keep)) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        for (int b = 0; b < nb; ++b) {
+            int rc = check_table(surf[b], S);
+            if (rc) return rc;
+            if (N[b] < 0 || (N[b] > 0 && (!y0[b] || !u0[b]))) return RTX_E_BADARG;
+        }
+        CK(cudaSetDevice(ctx->device));
+        return trace_batch_host<decltype(t)>(ctx, nb, surf, S, rot0, N, y0, u0, clip, keep, Y, U,
+                                             I, T, flags);
+    });
 }
 
 int rtx_trace_host(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, int dtype,
                    int64_t N, const void* y0, const void* u0, int clip, int keep, void* Y, void* U,
                    void* I, void* T, unsigned flags) {
     if (!ctx) return RTX_E_BADARG;
-    int rc = check_table(surf, S);
+    int rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || !y0 || !u0) return RTX_E_BADARG;
-    if (!valid_keep_dtype(keep, dtype)) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
-    if (dtype == RTX_F64)
-        return trace_host<double>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
-    return trace_host<float>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T, flags);
+    if (!valid_keep(keep)) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        if (N == 0) return 0;
+        CK(cudaSetDevice(ctx->device));
+        return trace_host<decltype(t)>(ctx, surf, S, rot0, N, y0, u0, clip, keep, Y, U, I, T,
+                                       flags);
+    });
 }
 
 int rtx_set_mask_output(rtx_ctx* ctx, uint32_t* dmask) {
@@ -1433,117 +1497,106 @@ int rtx_trace_gather(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
                      int64_t N, const void* y0, const void* u0, int clip, int npeers,
                      void* const* dst, void* const* dst_i, int64_t dst_offset, unsigned flags) {
     if (!ctx) return RTX_E_BADARG;
-    int rc = check_table(surf, S);
+    int rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || !y0 || !u0 || npeers < 1 || npeers > 8 || !dst || dst_offset < 0)
-        return RTX_E_BADARG;
-    if (!valid_keep_dtype(RTX_KEEP_LAST, dtype)) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    PeerDst pd;
-    pd.n = npeers;
-    pd.off = dst_offset;
-    pd.has_i = dst_i != nullptr;
-    pd.xy = (flags & RTX_GATHER_XY) != 0;
-    for (int k = 0; k < npeers; ++k) {
-        if (!dst[k] || (dst_i && !dst_i[k])) return RTX_E_BADARG;
-        pd.ptr[k] = dst[k];
-        if (dst_i) pd.ptr_i[k] = dst_i[k];
-    }
+    if (npeers < 1 || npeers > 8 || !dst || dst_offset < 0) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        if (N == 0) return 0;
+        PeerDst pd;
+        pd.n = npeers;
+        pd.off = dst_offset;
+        pd.has_i = dst_i != nullptr;
+        pd.xy = (flags & RTX_GATHER_XY) != 0;
+        for (int k = 0; k < npeers; ++k) {
+            if (!dst[k] || (dst_i && !dst_i[k])) return RTX_E_BADARG;
+            pd.ptr[k] = dst[k];
+            if (dst_i) pd.ptr_i[k] = dst_i[k];
+        }
+        CK(cudaSetDevice(ctx->device));
+        const long long ld = ((N + 127) / 128) * 128;  // only the gather destinations are written
+        return timed(ctx, [&] {
+            Launch<decltype(t)> L(surf, S, rot0, clip, RTX_KEEP_LAST, ld, flags);
+            L.peers = &pd;
+            return trace_registered(ctx, L, surf, N, y0, u0, nullptr, nullptr, nullptr, nullptr);
+        });
+    });
+}
+
+}  // extern "C"
+
+namespace {
+// rtx_selftest_*: uploads the K arrays `in` of in_bytes each, runs
+// launch(grid, d) with d[0..K) the device inputs and d[K] the output of
+// out_bytes over n items, and downloads that output to `out`
+template <size_t K, typename F>
+int selftest(rtx_ctx* ctx, long long n, const void* const (&in)[K], size_t in_bytes, void* out,
+             size_t out_bytes, F&& launch) {
     CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    const long long ld = ((N + 127) / 128) * 128;  // only the gather destinations are written
-    if (dtype == RTX_F64) {
-        Launch<double> L(surf, S, rot0, clip, RTX_KEEP_LAST, ld, flags);
-        L.peers = &pd;
-        rc = trace_registered(ctx, L, surf, N, y0, u0, nullptr, nullptr, nullptr, nullptr);
-    } else {
-        Launch<float> L(surf, S, rot0, clip, RTX_KEEP_LAST, ld, flags);
-        L.peers = &pd;
-        rc = trace_registered(ctx, L, surf, N, y0, u0, nullptr, nullptr, nullptr, nullptr);
-    }
-    if (rc) return rc;
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
+    DeviceBuf d[K + 1];
+    for (size_t k = 0; k < K; ++k) CK(d[k].alloc(in_bytes));
+    CK(d[K].alloc(out_bytes));
+    for (size_t k = 0; k < K; ++k)
+        CK(cudaMemcpyAsync(d[k].get(), in[k], in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    launch((unsigned)((n + 255) / 256), d);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, d[K].get(), out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
 
-int rtx_selftest_math(rtx_ctx* ctx, int64_t n, const double* a, const double* b, double* out) {
-    if (!ctx || n < 1 || !a || !b || !out) return RTX_E_BADARG;
+// rtx_moments, rtx_focus_moments: the 8 sums, zeroed, then added to by
+// launch(grid, sums) when N > 0, copied to m
+template <typename F>
+int moments(rtx_ctx* ctx, long long N, double* m, F&& launch) {
     CK(cudaSetDevice(ctx->device));
-    struct Bufs {  // freed on every return path
-        double *a = nullptr, *b = nullptr, *o = nullptr;
-        ~Bufs() {
-            cudaFree(a);
-            cudaFree(b);
-            cudaFree(o);
-        }
-    } d;
-    CK(cudaMalloc((void**)&d.a, n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.b, n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.o, 6 * n * sizeof(double)));
-    CK(cudaMemcpyAsync(d.a, a, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d.b, b, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    selftest_math_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.a, d.b, d.o, n);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, d.o, 6 * n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    Workspace& acc = ctx->ws[WS_MOMENTS];
+    int rc = reserve(acc, 8 * sizeof(double));
+    if (rc) return rc;
+    CK(cudaMemsetAsync(acc.p, 0, 8 * sizeof(double), ctx->stream));
+    if (N > 0) {
+        launch(cap_grid(ctx, (N + 255) / 256, 8), (double*)acc.p);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(m, acc.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_selftest_math(rtx_ctx* ctx, int64_t n, const double* a, const double* b, double* out) {
+    if (!ctx || n < 1 || !a || !b || !out) return RTX_E_BADARG;
+    const size_t v = n * sizeof(double);
+    return selftest(ctx, n, {a, b}, v, out, 6 * v, [&](unsigned grid, const DeviceBuf* d) {
+        selftest_math_kernel<<<grid, 256, 0, ctx->stream>>>(d[0].as<double>(), d[1].as<double>(),
+                                                            d[2].as<double>(), n);
+    });
 }
 
 int rtx_selftest_math2(rtx_ctx* ctx, int64_t n, const double* a, const double* b,
                        const double* c, double* out) {
     if (!ctx || n < 1 || !a || !b || !c || !out) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    struct Bufs {  // freed on every return path
-        double *a = nullptr, *b = nullptr, *c = nullptr, *o = nullptr;
-        ~Bufs() {
-            cudaFree(a);
-            cudaFree(b);
-            cudaFree(c);
-            cudaFree(o);
-        }
-    } d;
-    CK(cudaMalloc((void**)&d.a, n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.b, n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.c, n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.o, 7 * n * sizeof(double)));
-    CK(cudaMemcpyAsync(d.a, a, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d.b, b, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d.c, c, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    selftest_math2_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.a, d.b, d.c,
-                                                                               d.o, n);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, d.o, 7 * n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+    const size_t v = n * sizeof(double);
+    return selftest(ctx, n, {a, b, c}, v, out, 7 * v, [&](unsigned grid, const DeviceBuf* d) {
+        selftest_math2_kernel<<<grid, 256, 0, ctx->stream>>>(
+            d[0].as<double>(), d[1].as<double>(), d[2].as<double>(), d[3].as<double>(), n);
+    });
 }
 
 int rtx_moments(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* w,
                 const double* center, double* m) {
     if (!ctx || !y || !m || N < 0) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
     const double cx = center ? center[0] : 0.0, cy = center ? center[1] : 0.0;
-    CK(cudaMemsetAsync(ctx->d_moments, 0, 8 * sizeof(double), ctx->stream));
-    if (N > 0) {
-        long long blocks = (N + 255) / 256;
-        long long cap = (long long)ctx->sm_count * 8;
-        if (blocks > cap) blocks = cap;
-        if (dtype == RTX_F64)
-            moments_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                (const double*)y, (const double*)w, N, cx, cy, ctx->d_moments);
-        else if (dtype == RTX_F32)
-            moments_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                (const float*)y, (const float*)w, N, cx, cy, ctx->d_moments);
-        else
-            return RTX_E_BADARG;
-        ctx->launches++;
-        CK(cudaGetLastError());
-    }
-    CK(cudaMemcpyAsync(m, ctx->d_moments, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+    return dispatch(dtype, [&](auto t) {
+        using T = decltype(t);
+        return moments(ctx, N, m, [&](unsigned grid, double* acc) {
+            moments_kernel<T><<<grid, 256, 0, ctx->stream>>>((const T*)y, (const T*)w, N, cx, cy,
+                                                             acc);
+        });
+    });
 }
 
 }  // extern "C"
@@ -1588,6 +1641,19 @@ int launch_epi(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
     }
     return go(epi_kernel<T, false, RPT, MODE>);
 }
+
+// rtx_trace_reduce, rtx_trace_opd, rtx_trace_spot: the timed fused march of
+// N > 0 rays with the epilogue MODE, whose EpiParams members fill(p) sets
+template <int MODE, typename T, typename F>
+int trace_epi(rtx_ctx* ctx, T, const rtx_surface* surf, int S, const double* rot0, long long N,
+              const void* y0, const void* u0, int clip, unsigned flags, F&& fill) {
+    EpiParams<T> p;
+    memset(&p, 0, sizeof(p));
+    fill(p);
+    return timed(ctx, [&] {
+        return launch_epi<T, MODE>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
+    });
+}
 }  // namespace
 
 extern "C" {
@@ -1596,87 +1662,59 @@ int rtx_trace_reduce(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
                      int64_t N, const void* y0, const void* u0, int clip, const void* w,
                      const double* center, double* m, unsigned flags) {
     if (!ctx || !m) return RTX_E_BADARG;
-    int rc = check_table(surf, S);
+    int rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || !y0 || !u0) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    if (!ctx->d_epi) CK(cudaMalloc((void**)&ctx->d_epi, RTX_NMOMENTS * sizeof(double)));
-    CK(cudaMemsetAsync(ctx->d_epi, 0, RTX_NMOMENTS * sizeof(double), ctx->stream));
-    if (N > 0) {
-        CK(cudaEventRecord(ctx->k0, ctx->stream));
-        if (dtype == RTX_F64) {
-            EpiParams<double> p;
-            memset(&p, 0, sizeof(p));
-            p.w = (const double*)w;
-            for (int k = 0; k < 2; ++k) {
-                p.cy[k] = center ? center[k] : 0.0;
-                p.cu[k] = center ? center[2 + k] : 0.0;
-            }
-            p.out = ctx->d_epi;
-            rc = launch_epi<double, EPI_REDUCE>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-        } else {
-            EpiParams<float> p;
-            memset(&p, 0, sizeof(p));
-            p.w = (const float*)w;
-            for (int k = 0; k < 2; ++k) {
-                p.cy[k] = center ? center[k] : 0.0;
-                p.cu[k] = center ? center[2 + k] : 0.0;
-            }
-            p.out = ctx->d_epi;
-            rc = launch_epi<float, EPI_REDUCE>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-        }
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        CK(cudaSetDevice(ctx->device));
+        Workspace& acc = ctx->ws[WS_EPI];
+        int rc = reserve(acc, RTX_NMOMENTS * sizeof(double));
         if (rc) return rc;
-        CK(cudaEventRecord(ctx->k1, ctx->stream));
-        ctx->kernel_timed = true;
-    }
-    CK(cudaMemcpyAsync(m, ctx->d_epi, RTX_NMOMENTS * sizeof(double), cudaMemcpyDeviceToHost,
-                       ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+        CK(cudaMemsetAsync(acc.p, 0, RTX_NMOMENTS * sizeof(double), ctx->stream));
+        if (N > 0) {
+            rc = trace_epi<EPI_REDUCE>(ctx, t, surf, S, rot0, N, y0, u0, clip, flags, [&](auto& p) {
+                p.w = (const T*)w;
+                for (int k = 0; k < 2; ++k) {
+                    p.cy[k] = center ? center[k] : 0.0;
+                    p.cu[k] = center ? center[2 + k] : 0.0;
+                }
+                p.out = (double*)acc.p;
+            });
+            if (rc) return rc;
+        }
+        CK(cudaMemcpyAsync(m, acc.p, RTX_NMOMENTS * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        return 0;
+    });
 }
 
 int rtx_trace_opd(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, int dtype,
                   int64_t N, const void* y0, const void* u0, int clip, const rtx_opd* opd, void* A,
                   void* P, unsigned flags) {
     if (!ctx || !opd || !A || !P) return RTX_E_BADARG;
-    int rc = check_table(surf, S);
+    int rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || !y0 || !u0 || opd->radius == 0.0) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
-    if (N == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
-    auto fill = [&](auto& p) {
-        memset(&p, 0, sizeof(p));
-        p.infinite = opd->infinite;
-        for (int k = 0; k < 3; ++k) {
-            p.y0r[k] = opd->y0_ref[k];
-            p.u0r[k] = opd->u0_ref[k];
-            p.d[k] = opd->d[k];
-        }
-        for (int k = 0; k < 9; ++k) p.M[k] = opd->M[k];
-        p.n0 = opd->n0;
-        p.n_after = opd->n_after;
-        p.radius = opd->radius;
-    };
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    if (dtype == RTX_F64) {
-        EpiParams<double> p;
-        fill(p);
-        p.A = (double*)A;
-        p.P = (double*)P;
-        rc = launch_epi<double, EPI_OPD>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-    } else {
-        EpiParams<float> p;
-        fill(p);
-        p.A = (float*)A;
-        p.P = (float*)P;
-        rc = launch_epi<float, EPI_OPD>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-    }
-    if (rc) return rc;
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
-    return 0;
+    if (opd->radius == 0.0) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        if (N == 0) return 0;
+        CK(cudaSetDevice(ctx->device));
+        return trace_epi<EPI_OPD>(ctx, t, surf, S, rot0, N, y0, u0, clip, flags, [&](auto& p) {
+            p.infinite = opd->infinite;
+            for (int k = 0; k < 3; ++k) {
+                p.y0r[k] = opd->y0_ref[k];
+                p.u0r[k] = opd->u0_ref[k];
+                p.d[k] = opd->d[k];
+            }
+            for (int k = 0; k < 9; ++k) p.M[k] = opd->M[k];
+            p.n0 = opd->n0;
+            p.n_after = opd->n_after;
+            p.radius = opd->radius;
+            p.A = (T*)A;
+            p.P = (T*)P;
+        });
+    });
 }
 
 }  // extern "C"
@@ -1724,17 +1762,18 @@ int spot_to_dev(const rtx_spot* s, const uint64_t* counts, const double* extent,
 
 // the context's tally / extent accumulator, zeroed on the stream
 int spot_acc(rtx_ctx* ctx, SpotDev& d) {
-    if (!ctx->d_spot)
-        CK(cudaMalloc((void**)&ctx->d_spot, 5 * RTX_SPOT_MAX_PLANES * sizeof(unsigned long long)));
-    CK(cudaMemsetAsync(ctx->d_spot, 0, 5 * d.K * sizeof(unsigned long long), ctx->stream));
-    d.acc = ctx->d_spot;
+    Workspace& acc = ctx->ws[WS_SPOT];
+    int rc = reserve(acc, 5 * RTX_SPOT_MAX_PLANES * sizeof(unsigned long long));
+    if (rc) return rc;
+    CK(cudaMemsetAsync(acc.p, 0, 5 * d.K * sizeof(unsigned long long), ctx->stream));
+    d.acc = (unsigned long long*)acc.p;
     return 0;
 }
 
 int spot_finish(rtx_ctx* ctx, const SpotDev& d, uint64_t* tally, double* extent) {
     const int K = d.K;
     unsigned long long h[5 * RTX_SPOT_MAX_PLANES];
-    CK(cudaMemcpyAsync(h, ctx->d_spot, 5 * K * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+    CK(cudaMemcpyAsync(h, d.acc, 5 * K * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                        ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (tally)
@@ -1757,31 +1796,19 @@ int rtx_trace_spot(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* r
     int rc = spot_to_dev(spot, counts, extent, sd);
     if (rc) return rc;
     if (!ctx) return RTX_E_BADARG;
-    rc = check_table(surf, S);
+    rc = check_march(surf, S, N, y0, u0);
     if (rc) return rc;
-    if (N < 0 || !y0 || !u0) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    rc = spot_acc(ctx, sd);
-    if (rc) return rc;
-    if (N > 0) {
-        CK(cudaEventRecord(ctx->k0, ctx->stream));
-        if (dtype == RTX_F64) {
-            EpiParams<double> p;
-            memset(&p, 0, sizeof(p));
-            p.spot = sd;
-            rc = launch_epi<double, EPI_SPOT>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-        } else {
-            EpiParams<float> p;
-            memset(&p, 0, sizeof(p));
-            p.spot = sd;
-            rc = launch_epi<float, EPI_SPOT>(ctx, surf, S, rot0, N, y0, u0, clip, flags, p);
-        }
+    return dispatch(dtype, [&](auto t) -> int {
+        CK(cudaSetDevice(ctx->device));
+        int rc = spot_acc(ctx, sd);
         if (rc) return rc;
-        CK(cudaEventRecord(ctx->k1, ctx->stream));
-        ctx->kernel_timed = true;
-    }
-    return spot_finish(ctx, sd, tally, extent);
+        if (N > 0) {
+            rc = trace_epi<EPI_SPOT>(ctx, t, surf, S, rot0, N, y0, u0, clip, flags,
+                                     [&](auto& p) { p.spot = sd; });
+            if (rc) return rc;
+        }
+        return spot_finish(ctx, sd, tally, extent);
+    });
 }
 
 int rtx_spot_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* inc,
@@ -1790,27 +1817,23 @@ int rtx_spot_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void*
     int rc = spot_to_dev(spot, counts, extent, sd);
     if (rc) return rc;
     if (!ctx || N < 0 || !y || !inc) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    rc = spot_acc(ctx, sd);
-    if (rc) return rc;
-    if (N > 0) {
-        long long blocks = (N + 255) / 256;
-        const long long cap = (long long)ctx->sm_count * 8;
-        if (blocks > cap) blocks = cap;
-        CK(cudaEventRecord(ctx->k0, ctx->stream));
-        if (dtype == RTX_F64)
-            spot_rows_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                sd, (const double*)y, (const double*)inc, N);
-        else
-            spot_rows_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                sd, (const float*)y, (const float*)inc, N);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        CK(cudaEventRecord(ctx->k1, ctx->stream));
-        ctx->kernel_timed = true;
-    }
-    return spot_finish(ctx, sd, tally, extent);
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        CK(cudaSetDevice(ctx->device));
+        int rc = spot_acc(ctx, sd);
+        if (rc) return rc;
+        if (N > 0) {
+            const unsigned grid = cap_grid(ctx, (N + 255) / 256, 8);
+            rc = timed(ctx, [&] {
+                spot_rows_kernel<T><<<grid, 256, 0, ctx->stream>>>(sd, (const T*)y, (const T*)inc,
+                                                                   N);
+                ctx->launches++;
+                return (int)cudaGetLastError();
+            });
+            if (rc) return rc;
+        }
+        return spot_finish(ctx, sd, tally, extent);
+    });
 }
 
 }  // extern "C"
@@ -1873,16 +1896,12 @@ int aim_plan(rtx_ctx* ctx, const rtx_aim* spec, long long n_given, const void* y
     ctx->aim_total = d.M;
     if (rejects && d.M > 0) {
         const long long nb = (d.M + AIM_BLOCK - 1) / AIM_BLOCK;
-        if ((size_t)(nb + 1) * sizeof(long long) > ctx->d_aim_cap) {
-            if (ctx->d_aim_offsets) CK(cudaFree(ctx->d_aim_offsets));
-            ctx->d_aim_offsets = nullptr;
-            ctx->d_aim_cap = 0;
-            CK(cudaMalloc((void**)&ctx->d_aim_offsets, (size_t)(nb + 1) * sizeof(long long)));
-            ctx->d_aim_cap = (size_t)(nb + 1) * sizeof(long long);
-        }
-        int* d_counts = reinterpret_cast<int*>(ctx->d_aim_offsets);  // reused before the offsets
-        long long grid = nb < (long long)ctx->sm_count * 8 ? nb : (long long)ctx->sm_count * 8;
-        aim_count_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(d, (const double*)yp, d_counts, nb);
+        Workspace& ws = ctx->ws[WS_AIM];
+        rc = reserve(ws, (size_t)(nb + 1) * sizeof(long long));
+        if (rc) return rc;
+        int* d_counts = reinterpret_cast<int*>(ws.p);  // reused before the offsets
+        aim_count_kernel<<<cap_grid(ctx, nb, 8), 256, 0, ctx->stream>>>(d, (const double*)yp,
+                                                                        d_counts, nb);
         ctx->launches++;
         CK(cudaGetLastError());
         std::vector<int> counts((size_t)nb);
@@ -1897,7 +1916,7 @@ int aim_plan(rtx_ctx* ctx, const rtx_aim* spec, long long n_given, const void* y
         }
         ctx->aim_offsets[(size_t)nb] = acc;
         ctx->aim_total = acc;
-        CK(cudaMemcpyAsync(ctx->d_aim_offsets, ctx->aim_offsets.data(),
+        CK(cudaMemcpyAsync(ws.p, ctx->aim_offsets.data(),
                            (size_t)(nb + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
@@ -1922,75 +1941,52 @@ int rtx_aim_plan(rtx_ctx* ctx, const rtx_aim* spec, int64_t n_given, const void*
 int rtx_aim_rays(rtx_ctx* ctx, const rtx_aim* spec, int64_t n_given, const void* yp, int dtype,
                  int64_t first, int64_t count, void* y0, void* u0, void* yp_out) {
     if (!ctx || !spec || !y0 || !u0 || n_given < 0 || first < 0 || count < 0) return RTX_E_BADARG;
-    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    AimDev d;
-    int rc = aim_plan(ctx, spec, n_given, yp, d);
-    if (rc) return rc;
-    if (first + count > ctx->aim_total) return RTX_E_BADARG;
-    if (count == 0) return 0;
-    long long b0, b1;
-    const long long* d_off = nullptr;
-    if (ctx->aim_offsets.empty()) {
-        b0 = first / AIM_BLOCK;
-        b1 = (first + count + AIM_BLOCK - 1) / AIM_BLOCK;
-    } else {
-        const auto& off = ctx->aim_offsets;  // off[b] = rank of block b's first kept ray
-        const long long nb = (long long)off.size() - 1;
-        long long lo = 0, hi = nb;  // last block with off[b] <= first
-        while (lo + 1 < hi) {
-            const long long mid = (lo + hi) / 2;
-            if (off[(size_t)mid] <= first) lo = mid; else hi = mid;
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        CK(cudaSetDevice(ctx->device));
+        AimDev d;
+        int rc = aim_plan(ctx, spec, n_given, yp, d);
+        if (rc) return rc;
+        if (first + count > ctx->aim_total) return RTX_E_BADARG;
+        if (count == 0) return 0;
+        long long b0, b1;
+        const long long* d_off = nullptr;
+        if (ctx->aim_offsets.empty()) {
+            b0 = first / AIM_BLOCK;
+            b1 = (first + count + AIM_BLOCK - 1) / AIM_BLOCK;
+        } else {
+            const auto& off = ctx->aim_offsets;  // off[b] = rank of block b's first kept ray
+            const long long nb = (long long)off.size() - 1;
+            long long lo = 0, hi = nb;  // last block with off[b] <= first
+            while (lo + 1 < hi) {
+                const long long mid = (lo + hi) / 2;
+                if (off[(size_t)mid] <= first) lo = mid; else hi = mid;
+            }
+            b0 = lo;
+            b1 = b0;
+            while (b1 < nb && off[(size_t)b1] < first + count) ++b1;
+            d_off = (const long long*)ctx->ws[WS_AIM].p;
         }
-        b0 = lo;
-        b1 = b0;
-        while (b1 < nb && off[(size_t)b1] < first + count) ++b1;
-        d_off = ctx->d_aim_offsets;
-    }
-    long long grid = b1 - b0;
-    const long long cap = (long long)ctx->sm_count * 8;
-    if (grid > cap) grid = cap;
-    if (grid < 1) grid = 1;
-    if (dtype == RTX_F64)
-        aim_rays_kernel<double><<<(unsigned)grid, 256, 0, ctx->stream>>>(
-            d, (const double*)yp, d_off, b0, b1, first, count, (double*)y0, (double*)u0,
-            (double*)yp_out);
-    else
-        aim_rays_kernel<float><<<(unsigned)grid, 256, 0, ctx->stream>>>(
-            d, (const double*)yp, d_off, b0, b1, first, count, (float*)y0, (float*)u0,
-            (double*)yp_out);
-    ctx->launches++;
-    return (int)cudaGetLastError();
+        aim_rays_kernel<T><<<cap_grid(ctx, b1 - b0, 8), 256, 0, ctx->stream>>>(
+            d, (const double*)yp, d_off, b0, b1, first, count, (T*)y0, (T*)u0, (double*)yp_out);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
 }
 
 int rtx_focus_moments(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* inc,
                       const void* w, const double* center, double* m) {
     if (!ctx || !y || !inc || !m || N < 0) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
     double c[4] = {0, 0, 0, 0};
     if (center)
         for (int k = 0; k < 4; ++k) c[k] = center[k];
-    CK(cudaMemsetAsync(ctx->d_moments, 0, 8 * sizeof(double), ctx->stream));
-    if (N > 0) {
-        long long blocks = (N + 255) / 256;
-        long long cap = (long long)ctx->sm_count * 8;
-        if (blocks > cap) blocks = cap;
-        if (dtype == RTX_F64)
-            focus_moments_kernel<double><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                (const double*)y, (const double*)inc, (const double*)w, N, c[0], c[1], c[2], c[3],
-                ctx->d_moments);
-        else if (dtype == RTX_F32)
-            focus_moments_kernel<float><<<(unsigned)blocks, 256, 0, ctx->stream>>>(
-                (const float*)y, (const float*)inc, (const float*)w, N, c[0], c[1], c[2], c[3],
-                ctx->d_moments);
-        else
-            return RTX_E_BADARG;
-        ctx->launches++;
-        CK(cudaGetLastError());
-    }
-    CK(cudaMemcpyAsync(m, ctx->d_moments, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+    return dispatch(dtype, [&](auto t) {
+        using T = decltype(t);
+        return moments(ctx, N, m, [&](unsigned grid, double* acc) {
+            focus_moments_kernel<T><<<grid, 256, 0, ctx->stream>>>(
+                (const T*)y, (const T*)inc, (const T*)w, N, c[0], c[1], c[2], c[3], acc);
+        });
+    });
 }
 
 }  // extern "C"
@@ -2005,43 +2001,34 @@ int rtx_grid_linear(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, const v
     if (!ctx || M < 0 || T < 0 || T >= INT_MAX || n < 2 || n > 46340 || !gh || !out)
         return RTX_E_BADARG;
     if ((M > 0 && (!pts || !vals)) || (T > 0 && (!simplices || !transform))) return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
     const long long nn = (long long)n * n;
     int* claim = winner;
     if (!claim) {
-        if ((size_t)nn * sizeof(int) > ctx->winner_cap) {
-            if (ctx->d_winner) CK(cudaFree(ctx->d_winner));
-            ctx->d_winner = nullptr;
-            ctx->winner_cap = 0;
-            CK(cudaMalloc((void**)&ctx->d_winner, (size_t)nn * sizeof(int)));
-            ctx->winner_cap = (size_t)nn * sizeof(int);
-        }
-        claim = ctx->d_winner;
+        rc = reserve(ctx->ws[WS_WINNER], (size_t)nn * sizeof(int));
+        if (rc) return rc;
+        claim = (int*)ctx->ws[WS_WINNER].p;
     }
-    long long grid = (nn + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (grid > cap) grid = cap;
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    fill_i32_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(claim, nn, INT_MAX);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    if (T > 0) {
-        grid_claim_kernel<<<(unsigned)((T + 255) / 256), 256, 0, ctx->stream>>>(
-            (const double*)pts, M, simplices, (const double*)transform, T, (const double*)gh, n,
-            claim);
+    const unsigned grid = cap_grid(ctx, (nn + 255) / 256, 16);
+    return timed(ctx, [&] {
+        fill_i32_kernel<<<grid, 256, 0, ctx->stream>>>(claim, nn, INT_MAX);
         ctx->launches++;
         CK(cudaGetLastError());
-    }
-    grid_eval_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(
-        (const double*)vals, simplices, (const double*)transform, (const double*)gh, n, claim,
-        (double*)out);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
-    return 0;
+        if (T > 0) {
+            grid_claim_kernel<<<(unsigned)((T + 255) / 256), 256, 0, ctx->stream>>>(
+                (const double*)pts, M, simplices, (const double*)transform, T, (const double*)gh, n,
+                claim);
+            ctx->launches++;
+            CK(cudaGetLastError());
+        }
+        grid_eval_kernel<<<grid, 256, 0, ctx->stream>>>(
+            (const double*)vals, simplices, (const double*)transform, (const double*)gh, n, claim,
+            (double*)out);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
 }
 
 int rtx_psf_bytes(rtx_ctx* ctx, int n, int pad, size_t* bytes) {
@@ -2068,8 +2055,8 @@ int rtx_psf_bytes(rtx_ctx* ctx, int n, int pad, size_t* bytes) {
 
 int rtx_psf(rtx_ctx* ctx, int dtype, int n, const void* o, int pad, void* psf, double* stats) {
     if (!ctx || n < 1 || pad < 1 || !o || !psf) return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
     const CufftApi& fft = cufft_api();
     if (!fft.ok) return RTX_E_UNSUPPORTED;
     CK(cudaSetDevice(ctx->device));
@@ -2120,39 +2107,35 @@ int rtx_psf(rtx_ctx* ctx, int dtype, int n, const void* o, int pad, void* psf, d
     if (fft.set_stream(ctx->fft_plan, ctx->stream) != CUFFT_SUCCESS) return RTX_E_UNSUPPORTED;
     // partials (4 per block), the finite count, the 5 stats
     const size_t red_doubles = 4 * PSF_RED_BLOCKS + 1 + 5;
-    if (!ctx->d_psf_red) CK(cudaMalloc((void**)&ctx->d_psf_red, red_doubles * sizeof(double)));
-    double* part = ctx->d_psf_red;
+    rc = reserve(ctx->ws[WS_PSF_RED], red_doubles * sizeof(double));
+    if (rc) return rc;
+    double* part = (double*)ctx->ws[WS_PSF_RED].p;
     auto* count = reinterpret_cast<unsigned long long*>(part + 4 * PSF_RED_BLOCKS);
     double* d_stats = part + 4 * PSF_RED_BLOCKS + 1;
-    struct Grid {  // the complex grid is freed on every return path
-        double2* z = nullptr;
-        ~Grid() { if (z) cudaFree(z); }
-    } g;
-    if (cudaMalloc((void**)&g.z, zbytes) != cudaSuccess) {
+    DeviceBuf grid;  // the complex grid
+    if (grid.alloc(zbytes) != cudaSuccess) {
         cudaGetLastError();
-        g.z = nullptr;
         return RTX_E_NOMEM;
     }
+    double2* z = grid.as<double2>();
     const long long nn = (long long)n * n;
-    auto blocks = [&](long long items, long long per_sm) {
-        long long b = (items + 255) / 256, cap = (long long)ctx->sm_count * per_sm;
-        return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
-    };
     CK(cudaMemsetAsync(count, 0, sizeof(unsigned long long), ctx->stream));
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    count_finite_kernel<<<blocks(nn, 8), 256, 0, ctx->stream>>>((const double*)o, nn, count);
-    pupil_kernel<<<blocks(tot, 16), 256, 0, ctx->stream>>>((const double*)o, n, nx, ny, count, g.z);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    if (fft.exec_z2z(ctx->fft_plan, (cufftDoubleComplex*)g.z, (cufftDoubleComplex*)g.z,
-                     CUFFT_FORWARD) != CUFFT_SUCCESS)
-        return RTX_E_UNSUPPORTED;
-    intensity_kernel<<<PSF_RED_BLOCKS, 256, 0, ctx->stream>>>(g.z, nx, ny, (double*)psf, part);
-    psf_stats_kernel<<<1, 1, 0, ctx->stream>>>(part, PSF_RED_BLOCKS, count, d_stats);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
+    rc = timed(ctx, [&] {
+        count_finite_kernel<<<cap_grid(ctx, (nn + 255) / 256, 8), 256, 0, ctx->stream>>>(
+            (const double*)o, nn, count);
+        pupil_kernel<<<cap_grid(ctx, (tot + 255) / 256, 16), 256, 0, ctx->stream>>>(
+            (const double*)o, n, nx, ny, count, z);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+        if (fft.exec_z2z(ctx->fft_plan, (cufftDoubleComplex*)z, (cufftDoubleComplex*)z,
+                         CUFFT_FORWARD) != CUFFT_SUCCESS)
+            return RTX_E_UNSUPPORTED;
+        intensity_kernel<<<PSF_RED_BLOCKS, 256, 0, ctx->stream>>>(z, nx, ny, (double*)psf, part);
+        psf_stats_kernel<<<1, 1, 0, ctx->stream>>>(part, PSF_RED_BLOCKS, count, d_stats);
+        ctx->launches += 2;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
     if (stats)
         CK(cudaMemcpyAsync(stats, d_stats, 5 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -2163,8 +2146,8 @@ int rtx_psf_profiles(rtx_ctx* ctx, int dtype, int64_t nx, int64_t ny, const void
                      double c1, int64_t nbins, double* ee, double* lsf0, double* lsf1) {
     if (!ctx || !psf || nx < 1 || ny < 1 || !std::isfinite(c0) || !std::isfinite(c1))
         return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
     if (nx > INT64_MAX / 8 / ny) return RTX_E_BADARG;
     // np.bincount's length: 1 + the largest bin, which sits at a corner
     long long last = 0;
@@ -2180,35 +2163,21 @@ int rtx_psf_profiles(rtx_ctx* ctx, int dtype, int64_t nx, int64_t ny, const void
     const long long stride = nbins + nx + ny;
     // PROF_BLOCKS partial rows, their sum, the flag
     const size_t need = ((size_t)(PROF_BLOCKS + 1) * stride + 1) * sizeof(double);
-    if (need > ctx->prof_cap) {
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        if (need > free_b + ctx->prof_cap) return RTX_E_NOMEM;  // nothing allocated
-        if (ctx->d_prof) CK(cudaFree(ctx->d_prof));
-        ctx->d_prof = nullptr;
-        ctx->prof_cap = 0;
-        if (cudaMalloc((void**)&ctx->d_prof, need) != cudaSuccess) {
-            cudaGetLastError();
-            ctx->d_prof = nullptr;
-            return RTX_E_NOMEM;
-        }
-        ctx->prof_cap = need;
-    }
-    double* part = ctx->d_prof;
+    rc = reserve(ctx->ws[WS_PROF], need);
+    if (rc) return rc;
+    double* part = (double*)ctx->ws[WS_PROF].p;
     double* out = part + (long long)PROF_BLOCKS * stride;
     int* flag = reinterpret_cast<int*>(out + stride);
-    long long grid = (stride + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 8;
-    if (grid > cap) grid = cap;
+    const unsigned grid = cap_grid(ctx, (stride + 255) / 256, 8);
     CK(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
-    CK(cudaEventRecord(ctx->k0, ctx->stream));
-    profile_tiles_kernel<<<PROF_BLOCKS, PROF_WARPS * 32, 0, ctx->stream>>>(
-        (const double*)psf, nx, ny, c0, c1, nbins, part, stride, flag);
-    profile_combine_kernel<<<(unsigned)grid, 256, 0, ctx->stream>>>(part, PROF_BLOCKS, stride, out);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, ctx->stream));
-    ctx->kernel_timed = true;
+    rc = timed(ctx, [&] {
+        profile_tiles_kernel<<<PROF_BLOCKS, PROF_WARPS * 32, 0, ctx->stream>>>(
+            (const double*)psf, nx, ny, c0, c1, nbins, part, stride, flag);
+        profile_combine_kernel<<<grid, 256, 0, ctx->stream>>>(part, PROF_BLOCKS, stride, out);
+        ctx->launches += 2;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
     int h_flag = 0;
     CK(cudaMemcpyAsync(&h_flag, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     if (ee) CK(cudaMemcpyAsync(ee, out, nbins * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2274,55 +2243,26 @@ int rtx_delaunay_bytes(rtx_ctx* ctx, int64_t M, size_t* bytes) {
 
 int rtx_selftest_predicates(rtx_ctx* ctx, int64_t n, const double* pts, int* out) {
     if (!ctx || n < 1 || !pts || !out) return RTX_E_BADARG;
-    CK(cudaSetDevice(ctx->device));
-    struct Bufs {  // freed on every return path
-        double* q = nullptr;
-        int* o = nullptr;
-        ~Bufs() {
-            cudaFree(q);
-            cudaFree(o);
-        }
-    } d;
-    CK(cudaMalloc((void**)&d.q, 8 * n * sizeof(double)));
-    CK(cudaMalloc((void**)&d.o, 2 * n * sizeof(int)));
-    CK(cudaMemcpyAsync(d.q, pts, 8 * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    dt::selftest_predicates_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.q, n, d.o);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, d.o, 2 * n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+    return selftest(ctx, n, {pts}, 8 * n * sizeof(double), out, 2 * n * sizeof(int),
+                    [&](unsigned grid, const DeviceBuf* d) {
+                        dt::selftest_predicates_kernel<<<grid, 256, 0, ctx->stream>>>(
+                            d[0].as<double>(), n, d[1].as<int>());
+                    });
 }
 
 int rtx_delaunay(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, int64_t* T, int32_t* simplices,
                  int32_t* neighbors, void* transform) {
     if (!ctx || !pts || !T || !simplices) return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64 || M < 3 || M > DT_MAX_POINTS) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
+    if (M < 3 || M > DT_MAX_POINTS) return RTX_E_BADARG;
     CK(cudaSetDevice(ctx->device));
-    ctx->kernel_timed = false;  // until the call completes
-    const size_t need = dt_carve(nullptr, M, nullptr, nullptr);
-    if (need > ctx->dt_cap) {
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        if (need > free_b + ctx->dt_cap) return RTX_E_NOMEM;  // nothing allocated
-        if (ctx->d_dt) CK(cudaFree(ctx->d_dt));
-        ctx->d_dt = nullptr;
-        ctx->dt_cap = 0;
-        if (cudaMalloc(&ctx->d_dt, need) != cudaSuccess) {
-            cudaGetLastError();
-            ctx->d_dt = nullptr;
-            return RTX_E_NOMEM;
-        }
-        ctx->dt_cap = need;
-    }
+    rc = reserve(ctx->ws[WS_DT], dt_carve(nullptr, M, nullptr, nullptr));
+    if (rc) return rc;
     dt::Work w;
-    dt_carve(ctx->d_dt, M, pts, &w);
+    dt_carve(ctx->ws[WS_DT].p, M, pts, &w);
     cudaStream_t st = ctx->stream;
-    auto grid = [&](long long items) {
-        long long b = (items + 255) / 256, cap = (long long)ctx->sm_count * 16;
-        return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
-    };
+    const unsigned grid_m = cap_grid(ctx, (M + 255) / 256, 16);  // one thread per point
     unsigned cnt[dt::C_N];
     auto counters = [&]() -> int {  // launches so far checked, counters read back
         CK(cudaGetLastError());
@@ -2344,70 +2284,73 @@ int rtx_delaunay(rtx_ctx* ctx, int dtype, int64_t M, const void* pts, int64_t* T
     };
     auto relocate = [&]() -> int {
         CK(cudaMemsetAsync(w.cnt + dt::C_LEFT, 0, sizeof(unsigned), st));
-        dt::relocate_kernel<<<grid(M), 256, 0, st>>>(w, 2 * M + 16);
+        dt::relocate_kernel<<<grid_m, 256, 0, st>>>(w, 2 * M + 16);
         ctx->launches++;
         return counters();
     };
-    CK(cudaEventRecord(ctx->k0, st));
-    // validation and the seed triangle
-    CK(cudaMemsetAsync(w.cnt, 0, dt::C_N * sizeof(unsigned), st));
-    CK(cudaMemsetAsync(w.seed_key, 0xff, 8, st));
-    dt::lex_kernel<<<dt::LEX_BLOCKS, dt::LEX_THREADS, 0, st>>>(w);
-    dt::lex_final_kernel<<<1, 1, 0, st>>>(w);
-    CK(cudaGetLastError());
-    if (int rc = counters()) return rc;
-    if (cnt[dt::C_ERR]) return RTX_E_BADARG;  // non-finite or outside the predicates' domain
-    unsigned long long seed = 0;
-    dt::seed_kernel<<<grid(M), 256, 0, st>>>(w);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(&seed, w.seed_key, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    ctx->launches += 3;
-    if (seed == dt::NONE) return RTX_E_BADARG;  // all points collinear
-    fill_i32_kernel<<<grid(M), 256, 0, st>>>(w.loc, M, 0);
-    dt::init_kernel<<<1, 1, 0, st>>>(w);
-    ctx->launches += 2;
-    int tcur = 4, stamp = 1;
-    if (int rc = relocate()) return rc;
-    while (cnt[dt::C_LEFT]) {
-        CK(cudaMemsetAsync(w.pick, 0xff, (size_t)tcur * 8, st));
-        CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
-        dt::pick_kernel<<<grid(M), 256, 0, st>>>(w);
-        dt::claim_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
-        dt::decide_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
-        ctx->launches += 3;
-        int added = 0;
-        if (int rc = scan(tcur, &added)) return rc;
-        int m = stamp++, s = stamp++;
-        dt::split_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m, s);
-        tcur += 2 * added;
-        dt::fix_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m);
-        ctx->launches += 2;
-        for (;;) {
-            CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
-            CK(cudaMemsetAsync(w.cnt + dt::C_FLIPS, 0, sizeof(unsigned), st));
-            const int m2 = stamp++, s2 = stamp++;
-            dt::detect_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, s);
-            dt::flip_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, s, m2, s2);
-            dt::fix_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, m2);
-            ctx->launches += 3;
-            s = s2;
-            if (int rc = counters()) return rc;
-            if (!cnt[dt::C_FLIPS]) break;
-        }
-        if (int rc = relocate()) return rc;
-        if (cnt[dt::C_ERR]) return RTX_E_UNSUPPORTED;  // a broken invariant, never expected
-    }
-    // the finite triangles in slot order
-    dt::finite_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur);
-    ctx->launches++;
     int nfin = 0;
-    if (int rc = scan(tcur, &nfin)) return rc;
-    dt::output_kernel<<<grid(tcur), 256, 0, st>>>(w, tcur, simplices, neighbors, (double*)transform);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, st));
-    ctx->kernel_timed = true;
+    rc = timed(ctx, [&]() -> int {
+        // validation and the seed triangle
+        CK(cudaMemsetAsync(w.cnt, 0, dt::C_N * sizeof(unsigned), st));
+        CK(cudaMemsetAsync(w.seed_key, 0xff, 8, st));
+        dt::lex_kernel<<<dt::LEX_BLOCKS, dt::LEX_THREADS, 0, st>>>(w);
+        dt::lex_final_kernel<<<1, 1, 0, st>>>(w);
+        CK(cudaGetLastError());
+        if (int rc = counters()) return rc;
+        if (cnt[dt::C_ERR]) return RTX_E_BADARG;  // non-finite or outside the predicates' domain
+        unsigned long long seed = 0;
+        dt::seed_kernel<<<grid_m, 256, 0, st>>>(w);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(&seed, w.seed_key, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        ctx->launches += 3;
+        if (seed == dt::NONE) return RTX_E_BADARG;  // all points collinear
+        fill_i32_kernel<<<grid_m, 256, 0, st>>>(w.loc, M, 0);
+        dt::init_kernel<<<1, 1, 0, st>>>(w);
+        ctx->launches += 2;
+        int tcur = 4, stamp = 1;
+        if (int rc = relocate()) return rc;
+        while (cnt[dt::C_LEFT]) {
+            CK(cudaMemsetAsync(w.pick, 0xff, (size_t)tcur * 8, st));
+            CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
+            unsigned grid = cap_grid(ctx, (tcur + 255) / 256, 16);  // one thread per slot
+            dt::pick_kernel<<<grid_m, 256, 0, st>>>(w);
+            dt::claim_kernel<<<grid, 256, 0, st>>>(w, tcur);
+            dt::decide_kernel<<<grid, 256, 0, st>>>(w, tcur);
+            ctx->launches += 3;
+            int added = 0;
+            if (int rc = scan(tcur, &added)) return rc;
+            int m = stamp++, s = stamp++;
+            dt::split_kernel<<<grid, 256, 0, st>>>(w, tcur, m, s);
+            tcur += 2 * added;
+            grid = cap_grid(ctx, (tcur + 255) / 256, 16);
+            dt::fix_kernel<<<grid, 256, 0, st>>>(w, tcur, m);
+            ctx->launches += 2;
+            for (;;) {
+                CK(cudaMemsetAsync(w.vote, 0xff, (size_t)tcur * 8, st));
+                CK(cudaMemsetAsync(w.cnt + dt::C_FLIPS, 0, sizeof(unsigned), st));
+                const int m2 = stamp++, s2 = stamp++;
+                dt::detect_kernel<<<grid, 256, 0, st>>>(w, tcur, s);
+                dt::flip_kernel<<<grid, 256, 0, st>>>(w, tcur, s, m2, s2);
+                dt::fix_kernel<<<grid, 256, 0, st>>>(w, tcur, m2);
+                ctx->launches += 3;
+                s = s2;
+                if (int rc = counters()) return rc;
+                if (!cnt[dt::C_FLIPS]) break;
+            }
+            if (int rc = relocate()) return rc;
+            if (cnt[dt::C_ERR]) return RTX_E_UNSUPPORTED;  // a broken invariant, never expected
+        }
+        // the finite triangles in slot order
+        const unsigned grid = cap_grid(ctx, (tcur + 255) / 256, 16);
+        dt::finite_kernel<<<grid, 256, 0, st>>>(w, tcur);
+        ctx->launches++;
+        if (int rc = scan(tcur, &nfin)) return rc;
+        dt::output_kernel<<<grid, 256, 0, st>>>(w, tcur, simplices, neighbors, (double*)transform);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
     CK(cudaStreamSynchronize(st));
     *T = nfin;
     return 0;
@@ -2424,48 +2367,34 @@ int rtx_opd_points(rtx_ctx* ctx, int dtype, int64_t N, const void* A, const void
     if (!ctx || !A || !P || !pts || !vals || !M || !h || N < 1 || N >= (1ll << 31) || ref < 0 ||
         ref >= N || k == 0.0 || !std::isfinite(k))
         return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
     const int n = (int)N, nb = (n + dt::SCAN_THREADS - 1) / dt::SCAN_THREADS;
     // [max bits | block sums and the total | keep flags, ranked in place]
     const size_t bsum_off = 256, flag_off = bsum_off + ((size_t)(nb + 1) * 4 + 255) / 256 * 256;
-    const size_t need = flag_off + (size_t)n * 4;
-    if (need > ctx->opd_cap) {
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        if (need > free_b + ctx->opd_cap) return RTX_E_NOMEM;  // nothing allocated
-        if (ctx->d_opd) CK(cudaFree(ctx->d_opd));
-        ctx->d_opd = nullptr;
-        ctx->opd_cap = 0;
-        if (cudaMalloc(&ctx->d_opd, need) != cudaSuccess) {
-            cudaGetLastError();
-            ctx->d_opd = nullptr;
-            return RTX_E_NOMEM;
-        }
-        ctx->opd_cap = need;
-    }
-    auto* hbits = (unsigned long long*)ctx->d_opd;
-    int* bsum = (int*)((char*)ctx->d_opd + bsum_off);
-    int* flag = (int*)((char*)ctx->d_opd + flag_off);
+    rc = reserve(ctx->ws[WS_OPD], flag_off + (size_t)n * 4);
+    if (rc) return rc;
+    char* base = (char*)ctx->ws[WS_OPD].p;
+    auto* hbits = (unsigned long long*)base;
+    int* bsum = (int*)(base + bsum_off);
+    int* flag = (int*)(base + flag_off);
     const double *a = (const double*)A, *p = (const double*)P;
     cudaStream_t st = ctx->stream;
-    long long grid = (N + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (grid > cap) grid = cap;
+    const unsigned grid = cap_grid(ctx, (N + 255) / 256, 16);
     CK(cudaMemsetAsync(hbits, 0, 8, st));
-    CK(cudaEventRecord(ctx->k0, st));
-    opd_flag_kernel<<<(unsigned)grid, 256, 0, st>>>(a, p, N, ref, k, flag);
-    dt::scan_block_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum);
-    dt::scan_top_kernel<<<1, dt::SCAN_THREADS, 0, st>>>(bsum, nb);
-    // in place: each thread reads its own flag before the block scan and
-    // writes its rank after it
-    dt::scan_apply_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum, flag);
-    opd_scatter_kernel<<<(unsigned)grid, 256, 0, st>>>(a, p, N, ref, k, flag, pts, vals, hbits);
-    ctx->launches += 5;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, st));
-    ctx->kernel_timed = true;
+    rc = timed(ctx, [&] {
+        opd_flag_kernel<<<grid, 256, 0, st>>>(a, p, N, ref, k, flag);
+        dt::scan_block_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum);
+        dt::scan_top_kernel<<<1, dt::SCAN_THREADS, 0, st>>>(bsum, nb);
+        // in place: each thread reads its own flag before the block scan and
+        // writes its rank after it
+        dt::scan_apply_kernel<<<nb, dt::SCAN_THREADS, 0, st>>>(flag, n, bsum, flag);
+        opd_scatter_kernel<<<grid, 256, 0, st>>>(a, p, N, ref, k, flag, pts, vals, hbits);
+        ctx->launches += 5;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
     int count = 0;
     unsigned long long hb = 0;
     CK(cudaMemcpyAsync(&count, bsum + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2479,24 +2408,24 @@ int rtx_opd_points(rtx_ctx* ctx, int dtype, int64_t N, const void* A, const void
 int rtx_grid_range(rtx_ctx* ctx, int dtype, int64_t n, const void* o, int64_t* count, double* lo,
                    double* hi) {
     if (!ctx || n < 1 || !o || !count || !lo || !hi) return RTX_E_BADARG;
-    if (dtype == RTX_F32) return RTX_E_UNSUPPORTED;
-    if (dtype != RTX_F64) return RTX_E_BADARG;
+    int rc = fp64_only(dtype);
+    if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
-    if (!ctx->d_range) CK(cudaMalloc((void**)&ctx->d_range, 3 * sizeof(unsigned long long)));
+    rc = reserve(ctx->ws[WS_RANGE], 3 * sizeof(unsigned long long));
+    if (rc) return rc;
+    auto* d_acc = (unsigned long long*)ctx->ws[WS_RANGE].p;
     cudaStream_t st = ctx->stream;
-    long long grid = (n + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 8;
-    if (grid > cap) grid = cap;
-    CK(cudaMemsetAsync(ctx->d_range, 0, 3 * sizeof(unsigned long long), st));
-    CK(cudaMemsetAsync(ctx->d_range + 1, 0xff, sizeof(unsigned long long), st));  // min key: ~0
-    CK(cudaEventRecord(ctx->k0, st));
-    grid_range_kernel<<<(unsigned)grid, 256, 0, st>>>((const double*)o, n, ctx->d_range);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->k1, st));
-    ctx->kernel_timed = true;
+    const unsigned grid = cap_grid(ctx, (n + 255) / 256, 8);
+    CK(cudaMemsetAsync(d_acc, 0, 3 * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(d_acc + 1, 0xff, sizeof(unsigned long long), st));  // min key: ~0
+    rc = timed(ctx, [&] {
+        grid_range_kernel<<<grid, 256, 0, st>>>((const double*)o, n, d_acc);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
     unsigned long long acc[3];
-    CK(cudaMemcpyAsync(acc, ctx->d_range, sizeof(acc), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(acc, d_acc, sizeof(acc), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     auto value = [](unsigned long long key) {  // order_key's inverse
         const unsigned long long b = (key >> 63) ? key & ~0x8000000000000000ull : ~key;

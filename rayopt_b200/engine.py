@@ -65,6 +65,17 @@ def _code(dtype):
         raise TypeError("dtype must be float64 or float32, got %r" % (dtype,))
 
 
+def _rooms(dtype, arrays):
+    """(name, room in rays) of each (DeviceArray, values per ray) in `arrays`
+    (None entries are skipped); ValueError for one of another dtype"""
+    for name, (a, per_ray) in arrays.items():
+        if a is None:
+            continue
+        if np.dtype(a.dtype) != dtype:
+            raise ValueError("%s is %s but the rays are %s" % (name, np.dtype(a.dtype), dtype))
+        yield name, a.nbytes//(dtype.itemsize*per_ray)
+
+
 def _check_operands(dtype, N, **arrays):
     """The reductions and epilogues take their element type from the rays and
     read N rays from every other array: each (DeviceArray, values per ray)
@@ -73,12 +84,7 @@ def _check_operands(dtype, N, **arrays):
     dtype = np.dtype(dtype)
     if N < 0:
         raise ValueError("N must be >= 0, got %d" % N)
-    for name, (a, per_ray) in arrays.items():
-        if a is None:
-            continue
-        if np.dtype(a.dtype) != dtype:
-            raise ValueError("%s is %s but the rays are %s" % (name, np.dtype(a.dtype), dtype))
-        room = a.nbytes//(dtype.itemsize*per_ray)
+    for name, room in _rooms(dtype, arrays):
         if N > room:
             raise ValueError("N = %d rays but %s holds only %d" % (N, name, room))
 
@@ -90,12 +96,7 @@ def _check_trace_operands(dtype, N, rows, ld, outputs, mask=None, path_sum=None)
     launched) an operand of another element type or one too small for that."""
     dtype = np.dtype(dtype)
     _check_operands(dtype, N, path_sum=(path_sum, 1))
-    for name, (a, per_ray) in outputs.items():
-        if a is None:
-            continue
-        if np.dtype(a.dtype) != dtype:
-            raise ValueError("%s is %s but the rays are %s" % (name, np.dtype(a.dtype), dtype))
-        room = a.nbytes//(dtype.itemsize*per_ray)
+    for name, room in _rooms(dtype, outputs):
         if room < rows*ld:
             raise ValueError("%s holds %d rays but %d rows of pitch %d need %d"
                              % (name, room, rows, ld, rows*ld))
@@ -106,6 +107,11 @@ def _check_trace_operands(dtype, N, rows, ld, outputs, mask=None, path_sum=None)
         if mask.nbytes//4 < words:
             raise ValueError("N = %d rays need %d mask words but mask holds only %d"
                              % (N, words, mask.nbytes//4))
+
+
+def _rot0(rot0):
+    """the optional 3x3 launch rotation as 9 contiguous doubles"""
+    return None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
 
 
 def _given(yp):
@@ -339,6 +345,16 @@ class Engine:
             raise ValueError("surface table must be a non-empty 1-d record array")
         return table
 
+    def _march(self, table, y0, u0, N, clip, rot0, **operands):
+        """The prologue of the calls that march DEVICE launch rays: checks the
+        rays and `operands` as _check_operands does and returns the leading
+        arguments (ctx, table, S, rot0, dtype, N, y0, u0, clip) of the C call."""
+        table = self._table(table)
+        N = y0.shape[0] if N is None else int(N)
+        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3), **operands)
+        return (self.ctx, ptr(table), len(table), ptr(_rot0(rot0)), _code(y0.dtype), N, y0.ptr,
+                u0.ptr, int(bool(clip)))
+
     @staticmethod
     def _flags(exact, direct, rpt=0):
         return ((RTX_EXACT if exact else 0) | (RTX_STORE_DIRECT if direct else 0)
@@ -355,24 +371,20 @@ class Engine:
         the left-to-right sum of the stored t.  Operands of another dtype
         than the rays, or too small for rows x ld rays (N for path_sum,
         ceil(N/32) words for mask), raise ValueError."""
-        table = self._table(table)
-        dt = _code(y0.dtype)
-        N = y0.shape[0] if N is None else int(N)
+        if mask is None and path_sum is None and all(a is None for a in (Y, U, I, T)):
+            raise ValueError("nothing to store: pass an output array, a mask or a path sum")
+        args = self._march(table, y0, u0, N, clip, rot0)
+        S, N = args[2], args[5]
         first = next((a for a in (Y, U, I, T) if a is not None), None)
         if ld is None:
             ld = first.shape[1] if first is not None else (N + 63)//64*64
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         dp = lambda a: None if a is None else a.ptr  # noqa: E731
-        if mask is None and path_sum is None and all(a is None for a in (Y, U, I, T)):
-            raise ValueError("nothing to store: pass an output array, a mask or a path sum")
-        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
-        _check_trace_operands(y0.dtype, N, 1 if keep_last else len(table), int(ld),
+        _check_trace_operands(y0.dtype, N, 1 if keep_last else S, int(ld),
                               dict(Y=(Y, 3), U=(U, 3), I=(I, 3), T=(T, 1)), mask, path_sum)
         check(self.lib.rtx_set_mask_output(self.ctx, dp(mask)))
         check(self.lib.rtx_set_path_sum_output(self.ctx, dp(path_sum), int(path_sum_upto)))
         check(self.lib.rtx_trace(
-            self.ctx, ptr(table), len(table), ptr(r0), dt, N, y0.ptr, u0.ptr,
-            int(bool(clip)), RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL, ld,
+            *args, RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL, ld,
             dp(Y), dp(U), dp(I), dp(T), self._flags(exact, direct, rpt)))
 
     def trace_device_batch(self, tables, y0s, u0s, Ys, Us, Is, Ts, Ns=None, ld=None, clip=False,
@@ -404,9 +416,8 @@ class Engine:
             return (vp*nb)(*[vp(get(x)) for x in items])
         a_tab = arr(tabs, lambda t: t.ctypes.data)
         a_n = (C.c_int64*nb)(*Ns)
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         check(self.lib.rtx_trace_batch(
-            self.ctx, nb, C.cast(a_tab, vp), S, ptr(r0), dt, C.cast(a_n, vp),
+            self.ctx, nb, C.cast(a_tab, vp), S, ptr(_rot0(rot0)), dt, C.cast(a_n, vp),
             C.cast(arr(y0s, lambda a: a.ptr), vp), C.cast(arr(u0s, lambda a: a.ptr), vp),
             int(bool(clip)), RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL, ld,
             *[None if x is None else C.cast(arr(x, lambda a: a.ptr), vp) for x in (Ys, Us, Is, Ts)],
@@ -441,9 +452,8 @@ class Engine:
             if a.shape != shape or a.dtype != dtype or not a.flags.c_contiguous:
                 raise ValueError("output %r must be C-contiguous %s %r" % (k, dtype, shape))
             res.append(a)
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         check(self.lib.rtx_trace_host(
-            self.ctx, ptr(table), len(table), ptr(r0), dt, N, ptr(y0), ptr(u0),
+            self.ctx, ptr(table), len(table), ptr(_rot0(rot0)), dt, N, ptr(y0), ptr(u0),
             int(bool(clip)), RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL,
             ptr(res[0]), ptr(res[1]), ptr(res[2]), ptr(res[3]),
             self._flags(exact, direct, rpt)))
@@ -475,10 +485,9 @@ class Engine:
                 return None
             return C.cast((vp*nb)(*[vp(a.ctypes.data) for a in items]), vp)
         keep = [arr(tabs), arr(y0s), arr(u0s)] + [arr(outs[k]) for k in "yuit"]
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         check(self.lib.rtx_trace_batch_host(
-            self.ctx, nb, keep[0], S, ptr(r0), _code(dtype), C.cast((C.c_int64*nb)(*Ns), vp),
-            keep[1], keep[2], int(bool(clip)), RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL,
+            self.ctx, nb, keep[0], S, ptr(_rot0(rot0)), _code(dtype),
+            C.cast((C.c_int64*nb)(*Ns), vp), keep[1], keep[2], int(bool(clip)), RTX_KEEP_LAST if keep_last else RTX_KEEP_ALL,
             keep[3], keep[4], keep[5], keep[6], self._flags(exact, False)))
         return [tuple(None if outs[k] is None else outs[k][b] for k in "yuit") for b in range(nb)]
 
@@ -493,14 +502,12 @@ class Engine:
         `mask`, `path_sum`: the side outputs of trace_device for the shard's
         N rays; without them both are switched off, so that a gather never
         writes into buffers an earlier trace_device registered."""
-        table = self._table(table)
-        N = y0.shape[0] if N is None else int(N)
-        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
+        args = self._march(table, y0, u0, N, clip, rot0)
+        N = args[5]
         _check_trace_operands(y0.dtype, N, 1, N, {}, mask, path_sum)
         dp = lambda a: None if a is None else a.ptr  # noqa: E731
         check(self.lib.rtx_set_mask_output(self.ctx, dp(mask)))
         check(self.lib.rtx_set_path_sum_output(self.ctx, dp(path_sum), int(path_sum_upto)))
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
         arr = (C.c_void_p*len(dst_ptrs))(*[C.c_void_p(int(p)) for p in dst_ptrs])
         arr_i = None
         if dst_i_ptrs is not None:
@@ -509,8 +516,7 @@ class Engine:
             arr_i = C.cast((C.c_void_p*len(dst_ptrs))(*[C.c_void_p(int(p)) for p in dst_i_ptrs]),
                            C.c_void_p)
         check(self.lib.rtx_trace_gather(
-            self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
-            int(bool(clip)), len(dst_ptrs), C.cast(arr, C.c_void_p), arr_i, int(dst_offset),
+            *args, len(dst_ptrs), C.cast(arr, C.c_void_p), arr_i, int(dst_offset),
             self._flags(exact, False) | (_lib.RTX_GATHER_XY if xy else 0)))
 
     # ---- fused epilogues (no per-surface stores) -------------------------
@@ -520,16 +526,11 @@ class Engine:
         of `table` and return the 20 rms / refocus moments of that surface
         (include/rtx.h) -- one launch, no intercept is stored.  `center`:
         (y_x, y_y, u_x, u_y) guess centres (e.g. the chief ray's)."""
-        table = self._table(table)
-        N = y0.shape[0] if N is None else int(N)
-        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3), w=(w, 1))
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
+        args = self._march(table, y0, u0, N, clip, rot0, w=(w, 1))
         c = None if center is None else np.ascontiguousarray(center, np.float64).reshape(4)
         m = np.zeros(20)
         check(self.lib.rtx_trace_reduce(
-            self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
-            int(bool(clip)), None if w is None else w.ptr, ptr(c), ptr(m),
-            self._flags(exact, False)))
+            *args, None if w is None else w.ptr, ptr(c), ptr(m), self._flags(exact, False)))
         return m
 
     @staticmethod
@@ -569,19 +570,14 @@ class Engine:
     def trace_opd(self, table, y0, u0, spec, A, P, N=None, clip=False, rot0=None, exact=False):
         """rtx_trace_opd: `spec` a dict with the members of `struct rtx_opd`
         (include/rtx.h); A (N,), P (N,3) DeviceArrays.  Asynchronous."""
-        table = self._table(table)
-        N = y0.shape[0] if N is None else int(N)
-        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3), A=(A, 1), P=(P, 3))
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
+        args = self._march(table, y0, u0, N, clip, rot0, A=(A, 1), P=(P, 3))
         rec = np.zeros(1, OPD_DTYPE)
         for k in ("y0_ref", "u0_ref", "M", "d"):
             rec[k] = np.asarray(spec[k], float).reshape(rec[k].shape[1:])
         for k in ("n0", "n_after", "radius"):
             rec[k] = float(spec[k])
         rec["infinite"] = int(bool(spec["infinite"]))
-        check(self.lib.rtx_trace_opd(
-            self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
-            int(bool(clip)), ptr(rec), A.ptr, P.ptr, self._flags(exact, False)))
+        check(self.lib.rtx_trace_opd(*args, ptr(rec), A.ptr, P.ptr, self._flags(exact, False)))
 
     @staticmethod
     def _spot_outputs(spec, counts, extent):
@@ -607,14 +603,10 @@ class Engine:
         uint64 DeviceArray `counts` (added to; None: extent only) -- one
         launch, nothing per ray is stored.  Returns (tally (K,2): binned,
         non-finite; extent (K,3): max |q_x|, |q_y|, r, or None)."""
-        table = self._table(table)
-        N = y0.shape[0] if N is None else int(N)
-        _check_operands(y0.dtype, N, y0=(y0, 3), u0=(u0, 3))
+        args = self._march(table, y0, u0, N, clip, rot0)
         spec, tally, ext, cp = self._spot_outputs(spec, counts, extent)
-        r0 = None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
-        check(self.lib.rtx_trace_spot(
-            self.ctx, ptr(table), len(table), ptr(r0), _code(y0.dtype), N, y0.ptr, u0.ptr,
-            int(bool(clip)), ptr(spec), cp, ptr(tally), ptr(ext), self._flags(exact, False)))
+        check(self.lib.rtx_trace_spot(*args, ptr(spec), cp, ptr(tally), ptr(ext),
+                                      self._flags(exact, False)))
         return tally, ext
 
     def spot_rows(self, y, inc, spec, counts=None, N=None, extent=False):
