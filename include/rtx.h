@@ -408,6 +408,43 @@ int rtx_trace_reduce(rtx_ctx *ctx, const rtx_surface *surf, int S,
                      const double *center, double *m, unsigned flags);
 
 /*
+ * rtx_trace_reduce for many (surface table, launch bundle) items in ONE
+ * launch -- the tolerance analysis of thousands of perturbed lenses.
+ *   tables   host, nt*S records: table t is tables[t*S .. t*S+S-1]
+ *   rot0     shared by every table (NULL: none)
+ *   bundles  b < nb: DEVICE y0[b], u0[b] (N[b],3) of dtype; any number of
+ *            items may share one (the rays are read, never copied)
+ *   item i   marches bundle item_bundle[i] through table item_table[i] about
+ *            the guess centres centers[4i .. 4i+3] (host (nitems,4), or NULL
+ *            for 0), as rtx_trace_reduce's `center`
+ *   m        host (nitems, RTX_NMOMENTS): row i is item i's 20 moments, as
+ *            rtx_trace_reduce defines them with w = NULL (zeros for N = 0);
+ *            exactly nitems*20 doubles are written
+ * Each ray's state at surface S-1 is the last row rtx_trace stores for the
+ * same table, in every mode.  The sums are deterministic: item i's moments
+ * are the sum of its own 512-ray tiles in tile order, each tile summed by a
+ * warp shuffle tree and then its 8 warps in order (per-tile partials in the
+ * context and a second pass, no atomics).  So an item gives the same bits in
+ * every call and context, whatever the grid and whatever other items share
+ * the launch, in any order.  Error bound against the exact sum:
+ * (ceil(N/512) + 64) eps sum|term|.
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx, tables, N,
+ * y0, u0, item_table, item_bundle or m; nt, nb or nitems < 1; S outside
+ * 1..RTX_MAX_SURFACES; a table or bundle index out of range; N[b] < 0; NULL
+ * y0[b] or u0[b] with N[b] > 0; a bad dtype.  A record with n_asph >
+ * RTX_MAX_ASPH gives RTX_E_UNSUPPORTED, as in every march, and so does
+ * RTX_EXACT with RTX_F32.  The device tables, the items and the tile partials
+ * are kept in the context: RTX_E_NOMEM before allocating when they do not fit.
+ * Synchronous; rtx_last_kernel_ms covers the two kernels.
+ */
+int rtx_trace_reduce_many(rtx_ctx *ctx, int nt, const rtx_surface *tables, int S,
+                          const double *rot0, int dtype, int nb, const int64_t *N,
+                          const void *const *y0, const void *const *u0,
+                          int64_t nitems, const int32_t *item_table,
+                          const int32_t *item_bundle, const double *centers,
+                          int clip, double *m, unsigned flags);
+
+/*
  * The per-ray part of GeometricTrace.opd (rayopt/geometric_trace.py:101-131)
  * as the epilogue of the march to surface `after` (surf[S] = system[1:after+1]):
  *   A = sum_s t[s] - tj*n0 + ti*n_after,   P = y' + ti*u' - (0, 0, radius)

@@ -87,6 +87,7 @@ enum {
     WS_DT,       // rtx_delaunay: slots, adjacency and point-location workspace
     WS_OPD,      // rtx_opd_points: keep flags / ranks, block sums and max(|x|, |y|)
     WS_RANGE,    // rtx_grid_range: count, min key, max key
+    WS_MANY,     // rtx_trace_reduce_many: tables, items, tile sums, moments
     WS_COUNT
 };
 
@@ -1602,6 +1603,33 @@ int rtx_moments(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* w
 }  // extern "C"
 
 namespace {
+// one persistent wave of epi_kernel over `tiles` tiles of EPI_TILE rays, the
+// staged table of p.S records in dynamic shared memory
+template <typename T, int MODE>
+int launch_epi_kernel(rtx_ctx* ctx, unsigned flags, long long tiles, const EpiParams<T>& p) {
+    constexpr int RPT = 2, threads = 256;
+    static_assert(threads * RPT == EPI_TILE, "epi_kernel's tile");
+    size_t smem = (((size_t)p.S * sizeof(DevSurf<T>) + 127) & ~size_t(127)) + 16;
+    if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
+    auto go = [&](auto kern) -> int {
+        if (smem > 48 * 1024)
+            CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int occ = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
+        if (occ < 1) occ = 1;
+        long long grid = (long long)ctx->sm_count * occ;
+        if (grid > tiles) grid = tiles;
+        if (grid < 1) grid = 1;
+        kern<<<(unsigned)grid, threads, smem, ctx->stream>>>(p);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    };
+    if constexpr (sizeof(T) == 8) {
+        if (flags & RTX_EXACT) return go(epi_kernel<T, true, RPT, MODE>);
+    }
+    return go(epi_kernel<T, false, RPT, MODE>);
+}
+
 template <typename T, int MODE>
 int launch_epi(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, long long N,
                const void* y0, const void* u0, int clip, unsigned flags, EpiParams<T>& p) {
@@ -1617,29 +1645,8 @@ int launch_epi(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
     p.N = N;
     p.y0 = (const T*)y0;
     p.u0 = (const T*)u0;
-    const bool exact = (flags & RTX_EXACT) != 0;
-    if (exact && sizeof(T) == 4) return RTX_E_UNSUPPORTED;
-    constexpr int RPT = 2, threads = 256;
-    size_t smem = (((size_t)S * sizeof(DevSurf<T>) + 127) & ~size_t(127)) + 16;
-    if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
-    auto go = [&](auto kern) -> int {
-        if (smem > 48 * 1024)
-            CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int occ = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
-        if (occ < 1) occ = 1;
-        const long long tiles = (N + threads * RPT - 1) / (threads * RPT);
-        long long grid = (long long)ctx->sm_count * occ;
-        if (grid > tiles) grid = tiles;
-        if (grid < 1) grid = 1;
-        kern<<<(unsigned)grid, threads, smem, ctx->stream>>>(p);
-        ctx->launches++;
-        return (int)cudaGetLastError();
-    };
-    if constexpr (sizeof(T) == 8) {
-        if (exact) return go(epi_kernel<T, true, RPT, MODE>);
-    }
-    return go(epi_kernel<T, false, RPT, MODE>);
+    if ((flags & RTX_EXACT) && sizeof(T) == 4) return RTX_E_UNSUPPORTED;
+    return launch_epi_kernel<T, MODE>(ctx, flags, (N + EPI_TILE - 1) / EPI_TILE, p);
 }
 
 // rtx_trace_reduce, rtx_trace_opd, rtx_trace_spot: the timed fused march of
@@ -1686,6 +1693,110 @@ int rtx_trace_reduce(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
                            ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         return 0;
+    });
+}
+
+}  // extern "C"
+
+namespace {
+template <typename T>
+int trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
+                      const int64_t* N, const void* const* y0, const void* const* u0,
+                      long long nitems, const int32_t* item_table, const int32_t* item_bundle,
+                      const double* centers, int clip, double* m, unsigned flags) {
+    // the launch-wide tile list: item i owns tiles tile0 .. tile0 + ceil(N/512) - 1
+    std::vector<EpiItem> items((size_t)nitems);
+    long long tiles = 0;
+    for (long long i = 0; i < nitems; ++i) {
+        EpiItem& it = items[(size_t)i];
+        const int b = item_bundle[i];
+        it.y0 = y0[b];
+        it.u0 = u0[b];
+        it.N = N[b];
+        it.tile0 = tiles;
+        it.table = item_table[i];
+        for (int k = 0; k < 2; ++k) {
+            it.cy[k] = centers ? centers[4 * i + k] : 0.0;
+            it.cu[k] = centers ? centers[4 * i + 2 + k] : 0.0;
+        }
+        tiles += (N[b] + EPI_TILE - 1) / EPI_TILE;
+    }
+    // one workspace: tables | items | tile sums | moments
+    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t tb = up((size_t)nt * S * sizeof(DevSurf<T>)), ib = up(items.size() * sizeof(EpiItem));
+    const size_t mb = (size_t)nitems * RTX_NMOMENTS * sizeof(double);
+    if ((unsigned long long)tiles > (SIZE_MAX - tb - ib - mb) / (RTX_NMOMENTS * sizeof(double) + 1))
+        return RTX_E_NOMEM;
+    const size_t pb = up((size_t)tiles * RTX_NMOMENTS * sizeof(double));
+    CK(cudaSetDevice(ctx->device));
+    Workspace& ws = ctx->ws[WS_MANY];
+    int rc = reserve(ws, tb + ib + pb + mb);
+    if (rc) return rc;
+    unsigned char* base = (unsigned char*)ws.p;
+    DevSurf<T>* dtab = (DevSurf<T>*)base;
+    EpiItem* ditems = (EpiItem*)(base + tb);
+    double* part = (double*)(base + tb + ib);
+    double* dm = (double*)(base + tb + ib + pb);
+    std::vector<DevSurf<T>> host((size_t)nt * S);
+    for (size_t r = 0; r < host.size(); ++r) convert_surface<T>(tables[r], host[r]);
+    CK(cudaMemcpyAsync(dtab, host.data(), host.size() * sizeof(DevSurf<T>), cudaMemcpyHostToDevice,
+                       ctx->stream));
+    CK(cudaMemcpyAsync(ditems, items.data(), items.size() * sizeof(EpiItem),
+                       cudaMemcpyHostToDevice, ctx->stream));
+    EpiParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.table = dtab;
+    p.S = S;
+    p.clip = clip ? 1 : 0;
+    p.has_rot0 = rot0 != nullptr;
+    if (rot0)
+        for (int i = 0; i < 9; ++i) p.rot0[i] = (T)rot0[i];
+    p.items = ditems;
+    p.nitems = nitems;
+    p.tiles = tiles;
+    p.part = part;
+    rc = timed(ctx, [&]() -> int {
+        if (tiles > 0) {
+            int rc = launch_epi_kernel<T, EPI_MANY>(ctx, flags, tiles, p);
+            if (rc) return rc;
+        }
+        many_sum_kernel<<<cap_grid(ctx, (nitems * RTX_NMOMENTS + 255) / 256, 8), 256, 0,
+                          ctx->stream>>>(ditems, nitems, part, dm);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(m, dm, mb, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S,
+                          const double* rot0, int dtype, int nb, const int64_t* N,
+                          const void* const* y0, const void* const* u0, int64_t nitems,
+                          const int32_t* item_table, const int32_t* item_bundle,
+                          const double* centers, int clip, double* m, unsigned flags) {
+    if (!ctx || !tables || !N || !y0 || !u0 || !item_table || !item_bundle || !m)
+        return RTX_E_BADARG;
+    if (nt < 1 || nb < 1 || nitems < 1 || S < 1 || S > RTX_MAX_SURFACES) return RTX_E_BADARG;
+    for (int t = 0; t < nt; ++t) {
+        int rc = check_table(tables + (size_t)t * S, S);
+        if (rc) return rc;
+    }
+    for (int b = 0; b < nb; ++b)
+        if (N[b] < 0 || (N[b] > 0 && (!y0[b] || !u0[b]))) return RTX_E_BADARG;
+    for (long long i = 0; i < nitems; ++i)
+        if (item_table[i] < 0 || item_table[i] >= nt || item_bundle[i] < 0 ||
+            item_bundle[i] >= nb)
+            return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        if ((flags & RTX_EXACT) && sizeof(T) == 4) return RTX_E_UNSUPPORTED;
+        return trace_reduce_many<T>(ctx, nt, tables, S, rot0, N, y0, u0, nitems, item_table,
+                                    item_bundle, centers, clip, m, flags);
     });
 }
 

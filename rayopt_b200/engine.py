@@ -533,6 +533,63 @@ class Engine:
             *args, None if w is None else w.ptr, ptr(c), ptr(m), self._flags(exact, False)))
         return m
 
+    def trace_reduce_many(self, tables, bundles, items, centers=None, clip=False, rot0=None,
+                          exact=False):
+        """rtx_trace_reduce_many: `tables` (nt, S) records, `bundles` a list
+        of (y0, u0, N) DEVICE launch rays (N None: all rows), `items` (nitems,
+        2) of (table, bundle) indices, `centers` (nitems, 4) guess centres or
+        None.  Returns the (nitems, 20) moments of every item (w = 1) from one
+        launch; each row's bits depend on its own item only."""
+        tables = np.ascontiguousarray(tables, SURFACE_DTYPE)
+        if tables.ndim != 2 or tables.shape[0] < 1 or tables.shape[1] < 1:
+            raise ValueError("tables must be a non-empty (nt, S) record array")
+        if not bundles:
+            raise ValueError("no bundles")
+        dtype = np.dtype(bundles[0][0].dtype)
+        Ns = []
+        for y0, u0, N in bundles:
+            if np.dtype(y0.dtype) != dtype:
+                raise ValueError("every bundle must be %s, got %s" % (dtype, np.dtype(y0.dtype)))
+            N = y0.shape[0] if N is None else int(N)
+            _check_operands(dtype, N, y0=(y0, 3), u0=(u0, 3))
+            Ns.append(N)
+        items = np.ascontiguousarray(items, np.int64).reshape(-1, 2)
+        if len(items) < 1:
+            raise ValueError("no items")
+        if items.min() < 0 or items[:, 0].max() >= len(tables) or items[:, 1].max() >= len(bundles):
+            raise ValueError("an item's table or bundle index is out of range")
+        c = None
+        if centers is not None:
+            c = np.ascontiguousarray(centers, np.float64).reshape(len(items), 4)
+        it = np.ascontiguousarray(items[:, 0], np.int32)
+        ib = np.ascontiguousarray(items[:, 1], np.int32)
+        N = np.ascontiguousarray(Ns, np.int64)
+        y0s = (C.c_void_p*len(bundles))(*[b[0].ptr for b in bundles])
+        u0s = (C.c_void_p*len(bundles))(*[b[1].ptr for b in bundles])
+        m = np.zeros((len(items), 20))
+        check(self.lib.rtx_trace_reduce_many(
+            self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
+            len(bundles), ptr(N), y0s, u0s, len(items), ptr(it), ptr(ib), ptr(c), int(bool(clip)),
+            ptr(m), self._flags(exact, False)))
+        return m
+
+    @staticmethod
+    def rms_finite_from_moments(m):
+        """rms about the mean of the rays whose image x, y are finite, from
+        w = 1 moments: sqrt((m3 - (m1^2 + m2^2)/m0)/m0), written about the
+        guess centre as rms_from_moments is (cancellation free when the
+        centre lies within the spot).  Unlike GeometricTrace.rms it is not
+        NaN when rays are lost; where none is, it equals
+        rms_from_moments(m, unit_weights=True) bit for bit.  NaN when no ray
+        is finite.  `m` (20,) or (..., 20): returns a float or an array."""
+        m = np.asarray(m, np.float64)
+        n = m[..., 0]
+        with np.errstate(all="ignore"):
+            bx, by = m[..., 1]/n, m[..., 2]/n
+            r2 = m[..., 3] - 2*(bx*m[..., 1] + by*m[..., 2]) + (bx*bx + by*by)*n
+            r = np.where(n > 0, np.sqrt(np.maximum(r2/n, 0.)), np.nan)
+        return float(r) if r.ndim == 0 else r
+
     @staticmethod
     def rms_from_moments(m, unit_weights=False, about_center=False):
         """GeometricTrace.rms (rayopt/geometric_trace.py:171-183) from the

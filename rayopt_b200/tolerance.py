@@ -1,0 +1,334 @@
+"""Tolerance analysis on the device: trace many perturbed copies of a lens in
+one launch (rtx_trace_reduce_many) and reduce each to its spot moments.
+
+A perturbation is a list of parameters ``(j, kind)`` (j the index of a
+surface in the ``System``, >= 1) and a (V, P) array of deltas, one row per
+variant of the lens.  ``perturbed_tables`` applies them to the packed surface
+tables with ``pack_system``'s own expressions, so that a variant's records
+are the records of the ``System`` with the same change made.
+
+``tolerance`` aims every field and wavelength of the NOMINAL lens once
+(``system.pupil`` on the host, the launch rays generated in HBM) and marches
+that one object-space bundle through every variant: variants are not
+re-aimed, so a perturbation that moves the stop shows up as vignetting, and
+the stop and apertures of the perturbed lens decide which rays pass.
+"""
+import copy
+import math
+
+import numpy as np
+
+from .engine import Engine, default_engine
+from .surface_table import F_ROTATED, RTX_MAX_ASPH, SURFACE_DTYPE
+
+KINDS = ("curvature", "conic", "distance", "tilt_x", "tilt_y", "index") + tuple(
+    "asph%d" % i for i in range(RTX_MAX_ASPH))
+
+# rayopt's TransformMixin.update treats angles within np.allclose's default
+# absolute tolerance of 0 as no rotation at all
+_ANGLE_ATOL = 1e-8
+
+
+def _rot_rxyz(a):
+    """``rot_normal`` of a straight element with Euler angles `a` (rayopt's
+    TransformMixin.update, elements.py:120-154): the rotating-frame x-y-z
+    Euler matrix (axes "rxyz"), composed onto the identity as the reference
+    composes it"""
+    # rotating x-y-z: the angle sequence enters reversed and negated
+    si, sj, sk = math.sin(-a[2]), math.sin(-a[1]), math.sin(-a[0])
+    ci, cj, ck = math.cos(-a[2]), math.cos(-a[1]), math.cos(-a[0])
+    cc, cs = ci*ck, ci*sk
+    sc, ss = si*ck, si*sk
+    M = np.identity(3)
+    M[2, 2] = cj*ck
+    M[2, 1] = sj*sc - cs
+    M[2, 0] = sj*cc + ss
+    M[1, 2] = cj*sk
+    M[1, 1] = sj*ss + cc
+    M[1, 0] = sj*cs - sc
+    M[0, 2] = -sj
+    M[0, 1] = cj*si
+    M[0, 0] = cj*ci
+    return np.dot(np.eye(3), M)
+
+
+def _parse(params, S):
+    out = []
+    for j, kind in params:
+        if kind not in KINDS:
+            raise ValueError("unknown tolerance kind %r" % (kind,))
+        if int(j) != j or not 1 <= j <= S:
+            raise ValueError("surface %r is not in 1..%d" % (j, S))
+        out.append((int(j), kind))
+    return out
+
+
+def _move_distance(off_z, d):
+    """rayopt's ``distance += d`` on the offset's z (the element's length
+    along its direction, +z or, for a negative distance, -z)"""
+    return np.where(np.signbit(off_z), off_z - d, off_z + d)
+
+
+def perturbed_tables(tables, params, deltas):
+    """The (V, W, S) tables of V perturbed lenses from the nominal (W, S)
+    tables (one per wavelength, ``pack_system(system, l)``), the parameters
+    `params` [(j, kind)] and `deltas` (V, P).
+
+    kind       what changes in record j-1
+    curvature  c, then kc2
+    conic      k, then kc2
+    asph<i>    aspheric coefficient i and its derivative; a non-zero delta on
+               a surface without aspherics (or with fewer than i+1) makes it a
+               Newton surface of i+1 coefficients
+    distance   offset[2] (the element's distance); refused for an offset with
+               x or y != 0
+    tilt_x/_y  the Euler angles of an unrotated element (a tilt about the
+               surface vertex); refused for a rotated record
+    index      the index of the medium after surface j at every wavelength: n
+               and mu of record j-1, n0 and mu of record j; refused for the
+               last surface, a mirror, or a surface that does not bound a
+               medium (mu = 1 and n = n0) on either side
+
+    Raises ValueError before building anything."""
+    tables = np.asarray(tables, SURFACE_DTYPE)
+    if tables.ndim == 1:
+        tables = tables[None]
+    W, S = tables.shape
+    params = _parse(params, S)
+    deltas = np.asarray(deltas, np.float64)
+    if deltas.ndim != 2 or deltas.shape[1] != len(params):
+        raise ValueError("deltas must be (V, %d), got %s" % (len(params), deltas.shape))
+    for j, kind in params:
+        r = tables[:, j - 1]
+        if kind == "distance" and np.any(r["offset"][:, :2] != 0):
+            raise ValueError("surface %d is not on the axis of its predecessor" % j)
+        if kind in ("tilt_x", "tilt_y") and np.any(r["flags"] & F_ROTATED):
+            raise ValueError("surface %d is already rotated" % j)
+        if kind == "index":
+            if j == S:
+                raise ValueError("surface %d is the last: no medium follows it" % j)
+            for rr in (r, tables[:, j]):
+                if np.any(rr["mu"] == -1):
+                    raise ValueError("index of surface %d: a mirror bounds the medium" % j)
+                if np.any((rr["mu"] == 1) & (rr["n"] == rr["n0"])):
+                    raise ValueError("index of surface %d: the medium after it is not "
+                                     "bounded by two materials" % j)
+    V = deltas.shape[0]
+    out = np.repeat(tables[None], V, axis=0)
+    kc2_rows, mu_rows, angles = set(), set(), {}
+    for p, (j, kind) in enumerate(params):
+        r, d = j - 1, deltas[:, p, None]                       # (V, 1) over W
+        if kind == "curvature":
+            out["c"][:, :, r] += d
+            kc2_rows.add(r)
+        elif kind == "conic":
+            out["k"][:, :, r] += d
+            kc2_rows.add(r)
+        elif kind.startswith("asph"):
+            i = int(kind[4:])
+            out["asph"][:, :, r, i] += d
+            out["dasph"][:, :, r, i] = 2*(i + 1)*out["asph"][:, :, r, i]    # elements.py:472
+            na = out["n_asph"][:, :, r]
+            out["n_asph"][:, :, r] = np.where(d != 0, np.maximum(na, i + 1), na)
+        elif kind == "distance":
+            out["offset"][:, :, r, 2] = _move_distance(out["offset"][:, :, r, 2], d)
+        elif kind in ("tilt_x", "tilt_y"):
+            angles.setdefault(r, np.zeros((V, 3)))[:, int(kind == "tilt_y")] += deltas[:, p]
+        else:                                                  # index
+            out["n"][:, :, r] += d
+            out["n0"][:, :, r + 1] += d
+            mu_rows.update((r, r + 1))
+    for r in kc2_rows:
+        out["kc2"][:, :, r] = (1 + out["k"][:, :, r])*out["c"][:, :, r]**2   # elements.py:448,467
+    for r in mu_rows:                                          # Interface.get_n_mu, elements.py:283-289
+        mu = out["n0"][:, :, r]/out["n"][:, :, r]
+        out["mu"][:, :, r] = mu
+        out["muf"][:, :, r] = np.abs(mu)
+        out["sgn"][:, :, r] = np.sign(mu)
+        out["mu2m1"][:, :, r] = mu**2 - 1
+    for r, a in angles.items():
+        for v in range(V):
+            if np.all(np.abs(a[v]) <= _ANGLE_ATOL):
+                continue
+            out["rot"][v, :, r] = _rot_rxyz([float(x) for x in a[v]]).reshape(9)
+            out["flags"][v, :, r] |= F_ROTATED
+    return out
+
+
+def sensitivity_deltas(tol):
+    """(1 + 2P, P) deltas: row 0 the nominal lens, then +tol_p e_p and
+    -tol_p e_p for each parameter p in turn"""
+    tol = np.asarray(tol, np.float64).reshape(-1)
+    P = len(tol)
+    d = np.zeros((1 + 2*P, P))
+    d[1 + 2*np.arange(P), np.arange(P)] = tol
+    d[2 + 2*np.arange(P), np.arange(P)] = -tol
+    return d
+
+
+def monte_carlo_deltas(tol, trials, seed=None):
+    """(trials, P) deltas uniform in [-tol, tol] from np.random.default_rng(seed)"""
+    tol = np.asarray(tol, np.float64).reshape(-1)
+    return np.random.default_rng(seed).uniform(-tol, tol, (int(trials), len(tol)))
+
+
+def _chief(eng, table, rot0, y0, u0, exact):
+    """(y_x, y_y, u_x, u_y) of one launch ray at the last surface of `table`,
+    zeros where it does not get there"""
+    Y, _, I, _ = eng.trace(table, y0, u0, clip=True, rot0=rot0, keep_last=True, exact=exact,
+                           want=("y", "i"))
+    with np.errstate(all="ignore"):
+        c = np.r_[Y[0, 0, :2], I[0, 0, :2]/I[0, 0, 2]].astype(np.float64)
+    return c if np.all(np.isfinite(c)) else np.zeros(4)
+
+
+def launch_bundles(system, heights, wavelengths, nrays, distribution, engine):
+    """The nominal lens's launch rays of each (height, wavelength), generated
+    in HBM: a list of (y0, u0) DeviceArrays in height-major order and the
+    launch rays (2, 3) of each bundle's chief ray on the host"""
+    from .rays import aim_record, grid_spec
+    ref, grid = grid_spec(distribution, nrays)
+    if grid is None:
+        raise ValueError("distribution %r with %d rays is not generated on the device"
+                         % (distribution, nrays))
+    bundles, chiefs = [], []
+    for h in heights:
+        for l in wavelengths:
+            yo = (0, h)
+            z, p = system.pupil(yo, l=l)
+            rec = aim_record(system.object, yo, z, p, grid, False, system[0])
+            bundles.append(engine.aim_rays(rec))
+            cy, cu = engine.aim_rays(rec, first=ref, count=1)
+            chiefs.append((cy.download(), cu.download()))
+            cy.free(), cu.free()
+    return bundles, chiefs
+
+
+def _focus_bundles(system, l, engine):
+    """GeometricTrace.refocus's bundle in Analysis.run (analysis.py:84-88):
+    13 Radau rays on axis at `l`, unclipped, as given pupil coordinates.  The
+    reference weights them, and rtx_trace_reduce_many does not, so the rays
+    are split into one bundle per weight: [(weight, y0, u0)]"""
+    from rayopt.utils import pupil_distribution           # the reference's own helper
+    from .rays import aim_record
+    _, yp, weight = pupil_distribution("radau", 13)
+    yp = np.asarray(yp, np.float64)
+    w = np.ones(len(yp)) if weight is None else np.asarray(weight, np.float64)
+    z, p = system.pupil((0, 0.), l=l)
+    rec = aim_record(system.object, (0, 0.), z, p, None, False, system[0])
+    out = []
+    for wv in np.unique(w):
+        dyp = engine.to_device(yp[w == wv])
+        y0, u0 = engine.aim_rays(rec, yp=dyp)
+        dyp.free()
+        out.append((float(wv), y0, u0))
+    return out
+
+
+def focus_shifts(m, weights):
+    """GeometricTrace.refocus's shift from the unweighted moments m (..., G,
+    20) of G groups of rays that carry the weights `weights` (G,): the
+    weighted sums are sum_g w_g m_g"""
+    m = np.asarray(m, np.float64)
+    w = np.asarray(weights, np.float64)
+    tot = m.sum(-2)
+    tot[..., 13:20] = (m[..., 13:20]*w[:, None]).sum(-2)
+    return np.array([Engine.focus_shift_from_moments(t) for t in tot.reshape(-1, 20)]
+                    ).reshape(tot.shape[:-1])
+
+
+def _variant_chunk(tables_bytes_per_variant, tiles_per_variant, budget):
+    per = tables_bytes_per_variant + 160*tiles_per_variant + 1
+    return max(1, int(budget//per))
+
+
+def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, nrays=1000,
+              distribution="hexapolar", compensate=None, engine=None, exact=False, chunk=None):
+    """Spot rms, transmission and centroid of every perturbed lens at every
+    field height and wavelength, on the device.
+
+    `system` a rayopt ``System``; `params` [(j, kind)] and `deltas` (V, P) as
+    ``perturbed_tables``.  Each (height, wavelength) bundle is aimed once for
+    the NOMINAL lens and shared by all V variants (no re-aiming); the rays are
+    clipped by the perturbed lens.  ``compensate="focus"`` first refocuses
+    each variant as Analysis does (13 Radau rays on axis at wavelengths[0],
+    unclipped) and moves its image surface by the shift.  `chunk`: variants
+    per launch (default: as many as fit in 1 GiB of tables and tile sums);
+    the results do not depend on it.
+
+    Returns a dict: rms (V, H, W) about the mean of the rays that reach the
+    image, transmitted (V, H, W) the fraction that does, centroid (V, H, W,
+    2) relative to the nominal chief ray, moments (V, H, W, 20), focus (V,)
+    when compensated, and heights, wavelengths, params, deltas."""
+    from .surface_table import pack_system
+    if compensate not in (None, "focus"):
+        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
+    eng = engine or default_engine()
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    H, W = len(heights), len(wavelengths)
+    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
+    nominal = np.stack([t for t, _, _ in packs])
+    rot0 = packs[0][2]
+    S = nominal.shape[1]
+    params = list(params)
+    deltas = np.asarray(deltas, np.float64)
+    if deltas.ndim == 1:
+        deltas = deltas[None]
+    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
+    V = deltas.shape[0]
+    # System.pupil's result depends on the calls made before it: the focus
+    # bundle is aimed on a copy taken before any
+    fsys = copy.deepcopy(system) if compensate == "focus" else None
+    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
+    focus = fb = None
+    try:
+        centers = np.array([_chief(eng, nominal[b % W], rot0, y, u, exact)
+                            for b, (y, u) in enumerate(chiefs)])
+        dev = [(y, u, None) for y, u in bundles]
+        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
+        size = W*S*512                                         # device table bytes, FP64
+        step = int(chunk) if chunk else _variant_chunk(size, tiles, 2**30)
+        if step < 1:
+            raise ValueError("chunk must be >= 1")
+        if compensate == "focus":
+            fb = _focus_bundles(fsys, wavelengths[0], eng)
+            G = len(fb)
+            focus = np.empty(V)
+            for v0 in range(0, V, step):
+                t = perturbed_tables(nominal[:1], params, deltas[v0:v0 + step])[:, 0]
+                n = len(t)
+                items = np.stack(np.meshgrid(np.arange(n), np.arange(G), indexing="ij"),
+                                 -1).reshape(-1, 2)
+                m = eng.trace_reduce_many(t, [(y, u, None) for _, y, u in fb], items,
+                                          clip=False, rot0=rot0, exact=exact)
+                focus[v0:v0 + n] = focus_shifts(m.reshape(n, G, 20), [w for w, _, _ in fb])
+        moments = np.empty((V, H, W, 20))
+        vv, hh, ww = np.meshgrid(np.arange(V), np.arange(H), np.arange(W), indexing="ij")
+        for v0 in range(0, V, step):
+            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+            n = len(t)
+            if focus is not None:                              # system[-1].distance += shift
+                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
+                                                          focus[v0:v0 + n, None])
+            sl = slice(v0*H*W, (v0 + n)*H*W)
+            v, h, w = vv.reshape(-1)[sl] - v0, hh.reshape(-1)[sl], ww.reshape(-1)[sl]
+            items = np.stack([v*W + w, h*W + w], -1)
+            moments[v0:v0 + n] = eng.trace_reduce_many(
+                t.reshape(n*W, S), dev, items, centers[h*W + w], clip=True, rot0=rot0,
+                exact=exact).reshape(n, H, W, 20)
+    finally:
+        for y, u in bundles:
+            y.free(), u.free()
+        for _, y, u in fb or ():
+            y.free(), u.free()
+    m = moments
+    with np.errstate(all="ignore"):
+        out = dict(rms=Engine.rms_finite_from_moments(m), transmitted=m[..., 4]/m[..., 5],
+                   centroid=np.stack([m[..., 1]/m[..., 0], m[..., 2]/m[..., 0]], -1),
+                   moments=m, heights=np.asarray(heights, np.float64),
+                   wavelengths=np.asarray(wavelengths, np.float64), params=params,
+                   deltas=deltas)
+    if focus is not None:
+        out["focus"] = focus
+    return out
