@@ -65,7 +65,7 @@ struct Tuning {
     int lockstep = 1;         // CTA barrier per stored surface (STORE_WARP)
     int max_ctas_per_sm = 0;  // 0: whatever fits
     int max_clusters = -1;    // resident clusters of the clustered kernel (-1: MAX_STORE_CLUSTERS, 0: all that fit)
-    int tune = 1;             // TraceParams::tune bits (RTX_TUNE); 1 = L2 evict_first stores
+    bool prefetch = true;     // TraceParams::prefetch (RTX_TUNE bit 1 clears it)
 };
 
 // A device buffer of the context kept across calls: it grows (reserve) and
@@ -665,7 +665,7 @@ int launch_trace(rtx_ctx* ctx, const Launch<T>& L, cudaStream_t stream) {
         for (int i = 0; i < 9; ++i) p.rot0[i] = (T)L.rot0[i];
     p.ld = L.ld;
     p.lockstep = c.lockstep;
-    p.tune = ctx->tuning.tune;
+    p.prefetch = ctx->tuning.prefetch;
     if (const PeerDst* pd = L.peers) {
         p.npeer = pd->n;
         p.peer_off = pd->off;
@@ -1067,7 +1067,7 @@ int rtx_init(int device, rtx_ctx** out) {
     if (const char* e = getenv("RTX_LOCK")) tu.lockstep = atoi(e) != 0;
     if (const char* e = getenv("RTX_MAX_CTAS")) tu.max_ctas_per_sm = atoi(e);
     if (const char* e = getenv("RTX_MAX_CLUSTERS")) tu.max_clusters = atoi(e);
-    if (const char* e = getenv("RTX_TUNE")) tu.tune = atoi(e);
+    if (const char* e = getenv("RTX_TUNE")) tu.prefetch = !(atoi(e) & 2);
     *out = ctx;
     return 0;
 }

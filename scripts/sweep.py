@@ -6,8 +6,10 @@ configuration.  RTX_MAX_CLUSTERS (resident clusters of the clustered kernel,
 0: all that fit) is taken from the environment as set.
 usage: python scripts/sweep.py [--rays N] [--exact 0|1] cfg1 cfg2 ...
        cfg = rpt,store,warps,nbuf,lock,maxctas[,tune[,cluster]]   e.g. 2,1,8,2,1,0
-       (store 1: per-warp bulk stores, 2: per-CTA bulk stores; cluster: CTAs
-       per thread-block cluster of the per-CTA store kernel, 1: none)
+       (store 1: per-warp bulk stores, 2: per-CTA bulk stores; tune: RTX_TUNE,
+       of which only bit 1 (value 2: no input L2 prefetch) is read -- the bulk
+       stores always take the L2 evict_first policy; cluster: CTAs per
+       thread-block cluster of the per-CTA store kernel, 1: none)
 Build with RTX_TUNING_SPACE=1 for the full variant space."""
 import argparse, os, statistics, sys
 import numpy as np
