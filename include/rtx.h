@@ -593,7 +593,10 @@ int rtx_focus_moments(rtx_ctx *ctx, int dtype, int64_t N, const void *y,
  *   simplices (T,3) int32 and transform (T,3,2): Delaunay.simplices and
  *     Delaunay.transform as they are (degenerate simplices keep their NaNs and
  *     never cover a node),
- *   gh (n,) the grid axis, 2 <= n <= 46340: node (i, j) is (gh[i], gh[j]),
+ *   gh (n,) the grid axis, 2 <= n <= 46340: node (i, j) is (gh[i], gh[j]);
+ *     any strictly monotone finite axis, ascending or descending, evenly
+ *     spaced or not (each simplex finds its nodes by binary search on gh;
+ *     the axis is not checked, another one gives unspecified outputs),
  *   out (n,n) receives the values, NaN where no simplex covers the node,
  *   winner (n,n) int32 or NULL receives the covering simplex, the lowest
  *     index among the simplices that cover the node within scipy's tolerance
@@ -673,7 +676,11 @@ int rtx_psf_profiles(rtx_ctx *ctx, int dtype, int64_t nx, int64_t ny,
  *   simplices (T,3) int32, counter-clockwise,
  *   neighbors (T,3) int32 or NULL: the triangle opposite vertex k, -1 on the hull,
  *   transform (T,3,2) FP64 or NULL: {Tinv, r}, r the last vertex and Tinv the
- *     inverse (explicit 2x2 formula) of T = [v0 - r, v1 - r] as columns.
+ *     inverse (explicit 2x2 formula) of T = [v0 - r, v1 - r] as columns;
+ *     each entry within (3 rho + 3) DBL_EPSILON/2 of the exact inverse, rho =
+ *     (|t00 t11| + |t01 t10|)/|det|; a NaN row where the rounded determinant
+ *     is 0 (vertices collinear to rounding, never exactly), which covers no
+ *     node, as scipy's transform is NaN for a nearly singular simplex.
  * The triangulation is exactly Delaunay: orient2d and incircle are exact
  * (rtx_selftest_predicates), an edge is flipped only when its opposite vertex
  * is strictly inside the circumcircle, and the triangles cover exactly the

@@ -51,14 +51,32 @@ __global__ void fill_i32_kernel(int* __restrict__ a, long long n, int v) {
         a[k] = v;
 }
 
-// index range [lo, hi] of the grid nodes whose axis value may lie in
-// [vmin, vmax]: one node of margin on each side covers the rounding of the
-// division and scipy's eps, clamped to the grid
-__device__ __forceinline__ void node_range(double vmin, double vmax, double g0, double step, int n,
-                                           int& lo, int& hi) {
-    const double a = floor((vmin - g0) / step) - 1.0, b = ceil((vmax - g0) / step) + 1.0;
-    lo = a < 0.0 ? 0 : (a > n - 1 ? n : (int)a);
-    hi = b > n - 1 ? n - 1 : (b < 0.0 ? -1 : (int)b);
+// index range [lo, hi] of the grid nodes whose axis value lies in [vmin, vmax],
+// widened by the nearest node beyond each end and clamped to the grid.  The
+// axis gh is strictly monotone, ascending (s = 1) or descending (s = -1): in
+// the key s gh[i] it is ascending, and the box is [a, b] = s [vmin, vmax]
+// sorted.  The first node with key >= a is found by binary search, the last
+// one <= b by walking on from it (boxes are a few nodes wide).  A node that
+// passes scipy's 100-eps test lies within ~2 GRID_EPS (vmax - vmin) of the box
+// plus the rounding of its coordinates, far less than one spacing, so the one
+// node of margin covers every node a simplex can claim.
+__device__ __forceinline__ void node_range(double vmin, double vmax, const double* __restrict__ gh,
+                                           int n, double s, int& lo, int& hi) {
+    const double a = s > 0.0 ? vmin : -vmax, b = s > 0.0 ? vmax : -vmin;
+    int first = 0, len = n;  // first index with s gh[i] >= a, n if none
+    while (len > 0) {
+        const int half = len >> 1;
+        if (s * gh[first + half] < a) {
+            first += half + 1;
+            len -= half + 1;
+        } else {
+            len = half;
+        }
+    }
+    int last = first;  // first index with s gh[i] > b, n if none
+    while (last < n && s * gh[last] <= b) ++last;
+    lo = first > 0 ? first - 1 : 0;
+    hi = last < n ? last : n - 1;
 }
 
 // claim pass: one lane per simplex; boxes of more than GRID_WARP_NODES nodes
@@ -69,7 +87,7 @@ __global__ void __launch_bounds__(256) grid_claim_kernel(
     int* __restrict__ winner) {
     const long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
-    const double g0 = gh[0], step = (gh[n - 1] - gh[0]) / (double)(n - 1);
+    const double dir = gh[n - 1] < gh[0] ? -1.0 : 1.0;
     int i0 = 0, i1 = -1, j0 = 0, j1 = -1;
     const double* tr = transform + 6 * s;
     if (s < T && tr[0] == tr[0]) {  // NaN transform: degenerate, never a winner (as in scipy)
@@ -77,8 +95,8 @@ __global__ void __launch_bounds__(256) grid_claim_kernel(
         if (a >= 0 && a < M && b >= 0 && b < M && c >= 0 && c < M) {
             const double xa = pts[2 * a], xb = pts[2 * b], xc = pts[2 * c];
             const double ya = pts[2 * a + 1], yb = pts[2 * b + 1], yc = pts[2 * c + 1];
-            node_range(fmin(xa, fmin(xb, xc)), fmax(xa, fmax(xb, xc)), g0, step, n, i0, i1);
-            node_range(fmin(ya, fmin(yb, yc)), fmax(ya, fmax(yb, yc)), g0, step, n, j0, j1);
+            node_range(fmin(xa, fmin(xb, xc)), fmax(xa, fmax(xb, xc)), gh, n, dir, i0, i1);
+            node_range(fmin(ya, fmin(yb, yc)), fmax(ya, fmax(yb, yc)), gh, n, dir, j0, j1);
         }
     }
     const int wi = i1 >= i0 ? i1 - i0 + 1 : 0, wj = j1 >= j0 ? j1 - j0 + 1 : 0;

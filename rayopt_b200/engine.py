@@ -856,6 +856,9 @@ class Engine:
             raise ValueError("points must be (M, 2) FP64 and values (M,)")
         if gh.shape != (int(n),):
             raise ValueError("gh must be the (n,) grid axis")
+        step = np.diff(gh)
+        if not np.isfinite(gh).all() or not ((step > 0).all() or (step < 0).all()):
+            raise ValueError("gh must be finite and strictly monotone")
         n = int(n)
         ins = [values if dev_values else self.to_device(values), self.to_device(gh)]
         if not dev_points:
