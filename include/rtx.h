@@ -516,6 +516,57 @@ int rtx_spot_rows(rtx_ctx *ctx, int dtype, int64_t N, const void *y,
                   const void *inc, const rtx_spot *spot, uint64_t *counts,
                   uint64_t *tally, double *extent);
 
+/*
+ * Geometric OTF through focus: the Fourier transform of the spot diagram of
+ * stored rows y, inc (DEVICE (N,3) of dtype; a trace's y[at] and i[at]).
+ * Each ray's point at plane k is rtx_spot_rows' (FP64, every operation
+ * separately rounded, FP32 rows widened first):
+ *   d = y_xy - c,  u = i_xy / i_z,  q_k = (d + z[k] u) - o[k]
+ * A ray counts at plane k when both components of q_k are finite.  With
+ * nu_j = j*dnu (one rounded product), j < F, and a in {x, y}:
+ *   S[k,a,j] = sum over the counted rays of exp(-2 pi i nu_j q_k[a])
+ *   count[k] = number of counted rays;  OTF = S / count,  MTF = |OTF|
+ * S[k,a,0] is exactly count[k].  sums: host (K, 2, F, 2) doubles (re, im),
+ * count: host (K) int64; exactly K*2*F*2 doubles and K counts are written,
+ * zeros for N = 0.  Synchronous; rtx_last_kernel_ms covers both kernels.
+ *
+ * Deterministic: the rays are cut into slots of RTX_OTF_SLOT; each of the
+ * slot's 8 runs of RTX_OTF_SLOT/8 rays is summed in ray order, the runs in
+ * order, then the slot sums in slot order (a second kernel; no atomics).  The
+ * bits depend only on the rows and the spec, not on the grid, context or call.
+ * Each term starts from one sincospi for the first of a block of
+ * RTX_OTF_BLOCK frequencies and steps by the phasor exp(-2 pi i dnu q).
+ *
+ * Error bound, eps = 2^-52, Phi = max |nu_j q_k[a]| over the counted rays:
+ *   |S - S_exact| <= (D + 13 Phi + 5 RTX_OTF_BLOCK) eps count[k]
+ *   D = RTX_OTF_SLOT/8 + 8 + ceil(N / RTX_OTF_SLOT)   (the summation depth)
+ * per component.  13 Phi bounds the rounding of nu_j q and of the step
+ * phase, the recurrence's drift from fl(j dnu) and the step's error carried
+ * through RTX_OTF_BLOCK - 1 products (4 pi Phi); 5 RTX_OTF_BLOCK the 2 ulp of
+ * each sincospi component and the rounding of each complex product.
+ *
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx, spec, sums or
+ * count; NULL y or inc with N > 0; N < 0; a bad dtype; planes outside
+ * 1..RTX_OTF_MAX_PLANES, nfreq outside 1..RTX_OTF_MAX_FREQS; a non-finite
+ * dnu, c, z or o.  The slot sums are kept in the context
+ * (ceil(N/RTX_OTF_SLOT) (K*2*F*2 + K) doubles): RTX_E_NOMEM before
+ * allocating when they do not fit.
+ */
+#define RTX_OTF_MAX_PLANES 16
+#define RTX_OTF_MAX_FREQS  256
+#define RTX_OTF_SLOT       16384 /* rays per slot of the deterministic sum */
+#define RTX_OTF_BLOCK      16    /* frequencies per sincospi */
+typedef struct rtx_otf {
+    int32_t planes, nfreq;            /* K in 1..16, F in 1..256 */
+    double dnu;                       /* nu_j = j*dnu */
+    double c[2];                      /* subtracted from y_xy first */
+    double z[RTX_OTF_MAX_PLANES];     /* defocus distances */
+    double o[RTX_OTF_MAX_PLANES][2];  /* per-plane offsets subtracted last */
+} rtx_otf;
+size_t rtx_sizeof_otf(void);
+int rtx_otf_rows(rtx_ctx *ctx, int dtype, int64_t N, const void *y, const void *inc,
+                 const rtx_otf *spec, double *sums, int64_t *count);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

@@ -15,6 +15,7 @@ from .lazy import LazyRows, ResidentMixin, ResidentTrace  # noqa: F401
 from ._lib import RtxError  # noqa: F401
 from .spot import spots  # noqa: F401
 from .opd import opds  # noqa: F401
+from .mtf import geometric_mtf  # noqa: F401
 from .tolerance import (tolerance, perturbed_tables, sensitivity_deltas,  # noqa: F401
                         monte_carlo_deltas)
 

@@ -23,6 +23,7 @@ SYMBOLS = {
     "rtx_sizeof_aim": (_sz, []),
     "rtx_sizeof_opd": (_sz, []),
     "rtx_sizeof_spot": (_sz, []),
+    "rtx_sizeof_otf": (_sz, []),
     "rtx_device_count": (_i, []),
     "rtx_strerror": (C.c_char_p, [_i]),
     "rtx_surface_finalize": (_i, [_vp, _i, _vp]),
@@ -64,6 +65,7 @@ SYMBOLS = {
     "rtx_trace_opd": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_spot": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _vp, _u]),
     "rtx_spot_rows": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rtx_otf_rows": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),
@@ -116,10 +118,11 @@ def load():
     if lib.rtx_sizeof_aim() != aim_dtype().itemsize:
         raise RtxError("rtx_aim layout mismatch: C %d, numpy %d" % (
             lib.rtx_sizeof_aim(), aim_dtype().itemsize))
-    from .engine import SPOT_DTYPE
-    if lib.rtx_sizeof_spot() != SPOT_DTYPE.itemsize:
-        raise RtxError("rtx_spot layout mismatch: C %d, numpy %d" % (
-            lib.rtx_sizeof_spot(), SPOT_DTYPE.itemsize))
+    from .engine import OTF_DTYPE, SPOT_DTYPE
+    for name, dt in (("spot", SPOT_DTYPE), ("otf", OTF_DTYPE)):
+        if getattr(lib, "rtx_sizeof_" + name)() != dt.itemsize:
+            raise RtxError("rtx_%s layout mismatch: C %d, numpy %d" % (
+                name, getattr(lib, "rtx_sizeof_" + name)(), dt.itemsize))
     _lib = lib
     return lib
 

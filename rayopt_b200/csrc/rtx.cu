@@ -88,6 +88,7 @@ enum {
     WS_OPD,      // rtx_opd_points: keep flags / ranks, block sums and max(|x|, |y|)
     WS_RANGE,    // rtx_grid_range: count, min key, max key
     WS_MANY,     // rtx_trace_reduce_many: tables, items, tile sums, moments
+    WS_OTF,      // rtx_otf_rows: slot sums, then the call's sums and counts
     WS_COUNT
 };
 
@@ -977,6 +978,7 @@ size_t rtx_sizeof_surface(void) { return sizeof(rtx_surface); }
 size_t rtx_sizeof_aim(void) { return sizeof(rtx_aim); }
 size_t rtx_sizeof_opd(void) { return sizeof(rtx_opd); }
 size_t rtx_sizeof_spot(void) { return sizeof(rtx_spot); }
+size_t rtx_sizeof_otf(void) { return sizeof(rtx_otf); }
 
 int rtx_device_count(void) {
     int n = 0;
@@ -1944,6 +1946,71 @@ int rtx_spot_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void*
             if (rc) return rc;
         }
         return spot_finish(ctx, sd, tally, extent);
+    });
+}
+
+int rtx_otf_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* inc,
+                 const rtx_otf* spec, double* sums, int64_t* count) {
+    if (!ctx || !spec || !sums || !count || N < 0 || (N > 0 && (!y || !inc)))
+        return RTX_E_BADARG;
+    if (dtype != RTX_F64 && dtype != RTX_F32) return RTX_E_BADARG;
+    const int K = spec->planes, F = spec->nfreq;
+    if (K < 1 || K > RTX_OTF_MAX_PLANES || F < 1 || F > RTX_OTF_MAX_FREQS) return RTX_E_BADARG;
+    bool finite = std::isfinite(spec->dnu) && std::isfinite(spec->c[0]) &&
+                  std::isfinite(spec->c[1]);
+    for (int k = 0; k < K; ++k)
+        finite = finite && std::isfinite(spec->z[k]) && std::isfinite(spec->o[k][0]) &&
+                 std::isfinite(spec->o[k][1]);
+    if (!finite) return RTX_E_BADARG;
+    const int row = K * 2 * F * 2 + K;  // a slot's sums, then its counts
+    const long long slots = (N + RTX_OTF_SLOT - 1) / RTX_OTF_SLOT;
+    if (slots == 0) {
+        memset(sums, 0, (size_t)(row - K) * sizeof(double));
+        memset(count, 0, (size_t)K * sizeof(int64_t));
+        return 0;
+    }
+    OtfDev d;
+    memset(&d, 0, sizeof(d));
+    d.K = K;
+    d.F = F;
+    d.units = K * 2 * ((F + OTF_B - 1) / OTF_B);
+    d.groups = (d.units + 31) / 32;
+    d.dnu = spec->dnu;
+    d.c[0] = spec->c[0];
+    d.c[1] = spec->c[1];
+    for (int k = 0; k < K; ++k) {
+        d.z[k] = spec->z[k];
+        d.o[k][0] = spec->o[k][0];
+        d.o[k][1] = spec->o[k][1];
+    }
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        CK(cudaSetDevice(ctx->device));
+        Workspace& ws = ctx->ws[WS_OTF];
+        const size_t per = (size_t)row * sizeof(double);
+        if ((unsigned long long)slots >= SIZE_MAX / per - 1) return RTX_E_NOMEM;
+        int rc = reserve(ws, (size_t)(slots + 1) * per);
+        if (rc) return rc;
+        d.part = (double*)ws.p;
+        double* out = d.part + slots * row;
+        const long long items = slots * d.groups;
+        rc = timed(ctx, [&] {
+            otf_rows_kernel<T><<<cap_grid(ctx, items, 2), 256, 0, ctx->stream>>>(
+                d, (const T*)y, (const T*)inc, N, items);
+            ctx->launches++;
+            int rc = (int)cudaGetLastError();
+            if (rc) return rc;
+            otf_sum_kernel<<<(row + 255) / 256, 256, 0, ctx->stream>>>(d.part, row, slots, out);
+            ctx->launches++;
+            return (int)cudaGetLastError();
+        });
+        if (rc) return rc;
+        std::vector<double> h((size_t)row);
+        CK(cudaMemcpyAsync(h.data(), out, per, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        memcpy(sums, h.data(), (size_t)(row - K) * sizeof(double));
+        for (int k = 0; k < K; ++k) count[k] = (int64_t)h[(size_t)(row - K + k)];
+        return 0;
     });
 }
 

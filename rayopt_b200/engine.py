@@ -51,6 +51,48 @@ def spot_spec(z, bins, range, center, radial=False, offsets=None):
     return rec
 
 
+# mirrors `struct rtx_otf` (include/rtx.h)
+OTF_MAX_PLANES, OTF_MAX_FREQS = 16, 256
+OTF_SLOT, OTF_BLOCK = 16384, 16      # RTX_OTF_SLOT, RTX_OTF_BLOCK
+OTF_DTYPE = np.dtype([("planes", "<i4"), ("nfreq", "<i4"), ("dnu", "<f8"), ("c", "<f8", (2,)),
+                      ("z", "<f8", (OTF_MAX_PLANES,)), ("o", "<f8", (OTF_MAX_PLANES, 2))],
+                     align=True)
+
+
+def otf_spec(z, dnu, nfreq, c, offsets=None):
+    """An rtx_otf record: defocus distances `z` (K,), frequencies
+    ``arange(nfreq)*dnu``, the centre `c` (2,) subtracted from the
+    intercepts and per-plane `offsets` (K, 2) or None.  Raises ValueError
+    for what rtx_otf_rows refuses: K outside 1..16, nfreq outside 1..256,
+    a non-finite dnu, c, z or offset."""
+    z = np.atleast_1d(np.asarray(z, np.float64))
+    K, F = len(z), int(nfreq)
+    if z.ndim != 1 or not 1 <= K <= OTF_MAX_PLANES:
+        raise ValueError("need 1..%d planes, got %d" % (OTF_MAX_PLANES, K))
+    if not 1 <= F <= OTF_MAX_FREQS:
+        raise ValueError("need 1..%d frequencies, got %d" % (OTF_MAX_FREQS, F))
+    o = np.zeros((K, 2)) if offsets is None else np.asarray(offsets, np.float64).reshape(K, 2)
+    c = np.asarray(c, np.float64).reshape(2)
+    dnu = float(dnu)
+    if not (np.isfinite(dnu) and np.isfinite(c).all() and np.isfinite(z).all()
+            and np.isfinite(o).all()):
+        raise ValueError("dnu, c, z and offsets must be finite")
+    rec = np.zeros(1, OTF_DTYPE)
+    rec["planes"], rec["nfreq"], rec["dnu"], rec["c"] = K, F, dnu, c
+    rec["z"][0, :K], rec["o"][0, :K] = z, o
+    return rec
+
+
+def otf_bound(spec, N, count, phi, chunks=1):
+    """The error bound of include/rtx.h on every component of S, per plane
+    (K,): ``(D + 13 phi + 5 RTX_OTF_BLOCK) eps count`` with the summation
+    depth D of N rays in one call, plus ``chunks - 1`` for calls added in
+    order; `phi` the largest |nu_j q| over the counted rays"""
+    slots = -(-int(N)//OTF_SLOT)
+    D = OTF_SLOT//8 + 8 + slots + chunks - 1
+    return (D + 13*np.asarray(phi, np.float64) + 5*OTF_BLOCK)*2.**-52*np.asarray(count)
+
+
 def spot_shape(spec):
     """(K, nx, ny) of a 2-D record, (K, nx) of a radial one"""
     s = spec[0]
@@ -675,6 +717,24 @@ class Engine:
         check(self.lib.rtx_spot_rows(self.ctx, _code(y.dtype), N, y.ptr, inc.ptr, ptr(spec), cp,
                                      ptr(tally), ptr(ext)))
         return tally, ext
+
+    otf_spec = staticmethod(otf_spec)
+
+    def otf_rows(self, y, inc, spec, N=None):
+        """rtx_otf_rows: the geometric OTF sums of stored DEVICE rows y, inc
+        (N,3) (a trace's y[at], i[at]) at the planes and frequencies of
+        `spec` (otf_spec).  Returns (S complex128 (K, 2, F): sum over the
+        counted rays of exp(-2 pi i nu q) per plane, axis (x, y) and
+        frequency; count int64 (K,): the rays with a finite point)."""
+        N = y.shape[0] if N is None else int(N)
+        _check_operands(y.dtype, N, y=(y, 3), inc=(inc, 3))
+        spec = np.ascontiguousarray(spec, OTF_DTYPE).reshape(1)
+        K, F = int(spec[0]["planes"]), int(spec[0]["nfreq"])
+        sums = np.zeros((max(K, 1), 2, max(F, 1), 2))
+        count = np.zeros(max(K, 1), np.int64)
+        check(self.lib.rtx_otf_rows(self.ctx, _code(y.dtype), N, y.ptr, inc.ptr, ptr(spec),
+                                    ptr(sums), ptr(count)))
+        return sums[..., 0] + 1j*sums[..., 1], count
 
     def ipc_export(self, darray):
         h = (C.c_ubyte*64)()

@@ -623,6 +623,32 @@ class ResidentMixin:
         return self._one_image(spot_images(eng, [(c, [part])], defocus, bins, range, radial,
                                            offsets, download))
 
+    # ---- geometric MTF through focus (the Fourier transform of spot_image)
+    def geometric_mtf(self, defocus=(0.,), dnu=None, nfreq=64, at=-1):
+        """The geometric OTF of the stored rows y[at], i[at] about y[at, ref]
+        at the planes `defocus` (rtx_otf_rows): the mean over the rays with a
+        finite point q of exp(-2 pi i nu q), per plane, axis (x, y) and
+        frequency ``arange(nfreq)*dnu`` (``dnu=None``: the last frequency is
+        1/airy_radius, as mtf.geometric_mtf).  A vignetted ref ray gives a
+        NaN centre, counts nothing and gives NaN.  Returns a dict: freq (F,),
+        z (K,), otf complex (K, 2, F), mtf = |otf|, count (K,) int64."""
+        from .engine import otf_spec
+        from .mtf import _otf, default_dnu
+        eng, d = self._engine(), self._dev
+        at = int(np.arange(self.length)[at])
+        ref = 0 if self.ref is None else int(self.ref)
+        z = np.atleast_1d(np.asarray(defocus, np.float64))
+        F = int(nfreq)
+        dnu = default_dnu(self.system, F) if dnu is None else float(dnu)
+        c = eng.download_rays(d["y"].rows(at), [ref])[0, :2].astype(np.float64)
+        spec = otf_spec(z, dnu, F, np.nan_to_num(c))
+        if np.isfinite(c).all():
+            S, count = eng.otf_rows(d["y"].rows(at), d["i"].rows(at), spec, N=self.nrays)
+        else:
+            S, count = np.zeros((len(z), 2, F), np.complex128), np.zeros(len(z), np.int64)
+        otf = _otf(S, count)
+        return dict(freq=np.arange(F)*dnu, z=z, otf=otf, mtf=np.abs(otf), count=count)
+
     @staticmethod
     def _one_image(out):
         out["counts"], out["tally"] = out["counts"][0], out["tally"][0]
