@@ -567,6 +567,86 @@ size_t rtx_sizeof_otf(void);
 int rtx_otf_rows(rtx_ctx *ctx, int dtype, int64_t N, const void *y, const void *inc,
                  const rtx_otf *spec, double *sums, int64_t *count);
 
+/* ---- lens-parameter derivatives of the image point ---------------------- */
+/*
+ * The image point q = (y_x, y_y) of every ray at surface S-1 and its exact
+ * derivatives J = dq/dp with respect to P lens parameters, from one march
+ * (forward-mode tangents; FP64 only).
+ *
+ * A parameter p is a list of moves: moves[m] for m in param_first[p] ..
+ * param_first[p+1]-1 is the derivative of the record surf[move_row[m]] with
+ * respect to p (every member the kernel reads: offset, rot, c, k, kc2, mu,
+ * muf, mu2m1, n0, asph, dasph; flags, n_asph, sgn and radius2 are ignored),
+ * so a parameter may move several rows (a pickup, a refractive index).
+ *
+ *  surf, S, rot0, y0, u0, N, clip  as rtx_trace (dtype must be RTX_F64)
+ *  P           1 .. RTX_MAX_PARAMS
+ *  param_first host, P+1 int32 offsets: param_first[0] = 0, strictly rising
+ *  move_row    host, param_first[P] rows in 0 .. S-1
+ *  moves       host, param_first[P] records
+ *  q           DEVICE (N, 2) doubles
+ *  J           DEVICE (P, 2, ld) doubles: J[(2p + a) ld + k] = dq_a/dp of ray
+ *              k; ld >= N; columns N .. ld-1 are not written
+ *
+ * q equals the last row rtx_trace stores for the same arguments (its x, y),
+ * bit for bit, in each mode (RTX_EXACT or not).  J is the derivative of that
+ * march with the intercept taken as the EXACT root of the surface (implicit
+ * differentiation at the primal hit point, not of Newton's iterate): there is
+ * no derivative through ray aiming, clipping decisions, the choice of an
+ * intercept branch or the Newton stopping rule.  The tangents are FP64 with
+ * fused multiply-adds in both modes.  A ray whose q is NaN has NaN
+ * derivatives; a finite q may have a non-finite derivative where the ray
+ * grazes a surface (rtx_jacobian_sums counts those).
+ *
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx, surf, y0,
+ * u0, param_first, move_row, moves, q or J; S outside 1..RTX_MAX_SURFACES;
+ * N < 0; P outside 1..RTX_MAX_PARAMS; param_first[0] != 0 or a parameter
+ * without moves (param_first not strictly rising); a move_row outside
+ * 0..S-1; a move with a non-zero mu, muf or mu2m1 on a row whose mu is 1
+ * (that row does not refract, so the march has no derivative with respect
+ * to them); ld < N; a dtype other than RTX_F64.  A record of surf with n_asph >
+ * RTX_MAX_ASPH gives RTX_E_UNSUPPORTED, as in every march.  The tangent
+ * records are kept in the context.  Asynchronous; rtx_last_kernel_ms covers
+ * the kernel.
+ */
+#define RTX_MAX_PARAMS 64
+int rtx_trace_jacobian(rtx_ctx *ctx, const rtx_surface *surf, int S,
+                       const double *rot0, int dtype, int64_t N, const void *y0,
+                       const void *u0, int clip, int P, const int32_t *param_first,
+                       const int32_t *move_row, const rtx_surface *moves, void *q,
+                       void *J, int64_t ld, unsigned flags);
+
+/*
+ * Gauss-Newton sums of rtx_trace_jacobian's q (DEVICE (N, 2)) and J (DEVICE
+ * (P, 2, ld)) about the centre c (host, 2 doubles, or NULL for 0), with
+ * d = fl(q - c).  A ray enters iff q and all of its 2P derivatives are
+ * finite.  out (host, W = 5 + 3P + P(P+1)/2 doubles), over the rays that
+ * enter:
+ *   out[0]              n
+ *   out[1..2]           sum d_x, sum d_y
+ *   out[3]              sum |d|^2
+ *   out[4 + 2a + x]     G_a = sum dq/dp_a           (a < P, x the axis)
+ *   out[4 + 2P + a]     H_a = sum d . dq/dp_a
+ *   out[4 + 3P + ...]   K_ab = sum dq/dp_a . dq/dp_b, a <= b, row-major
+ *                       packed upper triangle (P(P+1)/2 values)
+ *   out[W - 1]          rays with a finite q and a non-finite derivative
+ *                       (they do not enter)
+ * Deterministic: each RTX_JAC_SLOT-ray slot is summed in ray order by one
+ * thread per output, the slot sums then in slot order (a second kernel; no
+ * atomics), so the bits depend only on q, J and c.  Error bound against the
+ * exact sum of the same terms, eps = 2^-52:
+ *   |out - exact| <= (2 RTX_JAC_SLOT + ceil(N / RTX_JAC_SLOT)) eps sum|term|
+ * where the terms are the single products of d and J entries each output
+ * adds (two per ray for sum |d|^2, H and K).  Counts are exact.
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx or out; NULL
+ * q or J with N > 0; N < 0; P outside 1..RTX_MAX_PARAMS; ld < N.  The slot
+ * sums are kept in the context: RTX_E_NOMEM before allocating when they do
+ * not fit.  Synchronous; rtx_last_kernel_ms covers both kernels.
+ */
+#define RTX_JAC_SLOT 16384
+int rtx_jacobian_sums(rtx_ctx *ctx, int64_t N, int P, const void *q, const void *J,
+                      int64_t ld, const double *center, double *out);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

@@ -17,6 +17,7 @@ from .spot import spots  # noqa: F401
 from .opd import opds  # noqa: F401
 from .mtf import geometric_mtf  # noqa: F401
 from .tolerance import (tolerance, perturbed_tables, sensitivity_deltas,  # noqa: F401
-                        monte_carlo_deltas)
+                        monte_carlo_deltas, record_tangents)
+from .optimize import spot_jacobian, optimize_spot  # noqa: F401
 
 __version__ = "0.2.0"

@@ -66,6 +66,9 @@ SYMBOLS = {
     "rtx_trace_spot": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _vp, _u]),
     "rtx_spot_rows": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rtx_otf_rows": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "rtx_trace_jacobian": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp,
+                                _vp, _i64, _u]),
+    "rtx_jacobian_sums": (_i, [_vp, _i64, _i, _vp, _vp, _i64, _vp, _vp]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),

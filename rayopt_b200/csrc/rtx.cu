@@ -89,6 +89,8 @@ enum {
     WS_RANGE,    // rtx_grid_range: count, min key, max key
     WS_MANY,     // rtx_trace_reduce_many: tables, items, tile sums, moments
     WS_OTF,      // rtx_otf_rows: slot sums, then the call's sums and counts
+    WS_JAC,      // rtx_trace_jacobian: tangent records, their index, block first rows
+    WS_JSUM,     // rtx_jacobian_sums: slot sums, then the call's sums
     WS_COUNT
 };
 
@@ -2012,6 +2014,155 @@ int rtx_otf_rows(rtx_ctx* ctx, int dtype, int64_t N, const void* y, const void* 
         for (int k = 0; k < K; ++k) count[k] = (int64_t)h[(size_t)(row - K + k)];
         return 0;
     });
+}
+
+}  // extern "C"
+
+namespace {
+// a move record as the derivative of the DevSurf<double> members jac_kernel
+// reads, added to `d` (several moves of one parameter may share a row)
+void add_tangent(const rtx_surface& s, JacTan& d) {
+    for (int i = 0; i < 3; ++i) d.off[i] += s.offset[i];
+    for (int i = 0; i < 9; ++i) {
+        d.rot[i] += s.rot[i];
+        if (d.rot[i] != 0.0) d.has_rot = 1;
+    }
+    d.c += s.c;
+    d.k1 += s.k;
+    d.kc2 += s.kc2;
+    d.mu += s.mu;
+    d.muf += s.muf;
+    d.mu2m1 += s.mu2m1;
+    for (int i = 0; i < RTX_MAX_ASPH; ++i) {
+        d.asph[i] += s.asph[i];
+        d.dasph[i] += s.dasph[i];
+        if (d.asph[i] != 0.0 || d.dasph[i] != 0.0) d.n_asph = std::max(d.n_asph, i + 1);
+    }
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
+                       int dtype, int64_t N, const void* y0, const void* u0, int clip, int P,
+                       const int32_t* param_first, const int32_t* move_row,
+                       const rtx_surface* moves, void* q, void* J, int64_t ld, unsigned flags) {
+    if (!ctx || !param_first || !move_row || !moves || !q || !J) return RTX_E_BADARG;
+    if (!surf || S < 1 || S > RTX_MAX_SURFACES || N < 0 || !y0 || !u0) return RTX_E_BADARG;
+    if (dtype != RTX_F64 || P < 1 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
+    if (param_first[0] != 0) return RTX_E_BADARG;
+    for (int p = 0; p < P; ++p)
+        if (param_first[p + 1] <= param_first[p]) return RTX_E_BADARG;
+    for (int m = 0; m < param_first[P]; ++m) {
+        if (move_row[m] < 0 || move_row[m] >= S) return RTX_E_BADARG;
+        // a row with mu == 1 does not refract (elements.py:356): there is no
+        // refraction to differentiate with respect to mu, muf or mu2m1
+        const rtx_surface& mv = moves[m];
+        if (surf[move_row[m]].mu == 1.0 && (mv.mu != 0.0 || mv.muf != 0.0 || mv.mu2m1 != 0.0))
+            return RTX_E_BADARG;
+    }
+    int rc = check_table(surf, S);
+    if (rc) return rc;
+    if (N == 0) return 0;
+    // the tangent records: one per (parameter, moved row), their (P, S) index
+    // and the first moved row of each block of JAC_PB parameters
+    const int nblk = (P + JAC_PB - 1) / JAC_PB;
+    std::vector<int> idx((size_t)P * S, -1), first(nblk, S);
+    std::vector<JacTan> tan;
+    for (int p = 0; p < P; ++p)
+        for (int m = param_first[p]; m < param_first[p + 1]; ++m) {
+            int& k = idx[(size_t)p * S + move_row[m]];
+            if (k < 0) {
+                k = (int)tan.size();
+                tan.emplace_back();
+                memset(&tan.back(), 0, sizeof(JacTan));
+            }
+            add_tangent(moves[m], tan[(size_t)k]);
+            first[p / JAC_PB] = std::min(first[p / JAC_PB], (int)move_row[m]);
+        }
+    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t tb = up(tan.size() * sizeof(JacTan)), xb = up(idx.size() * sizeof(int));
+    CK(cudaSetDevice(ctx->device));
+    Workspace& ws = ctx->ws[WS_JAC];
+    rc = reserve(ws, tb + xb + first.size() * sizeof(int));
+    if (rc) return rc;
+    unsigned char* base = (unsigned char*)ws.p;
+    JacParams jp;
+    memset(&jp, 0, sizeof(jp));
+    jp.tan = (const JacTan*)base;
+    jp.idx = (const int*)(base + tb);
+    jp.first = (const int*)(base + tb + xb);
+    // pageable sources: each copy has left the host vector when it returns
+    CK(cudaMemcpyAsync(base, tan.data(), tan.size() * sizeof(JacTan), cudaMemcpyHostToDevice,
+                       ctx->stream));
+    CK(cudaMemcpyAsync(base + tb, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice,
+                       ctx->stream));
+    CK(cudaMemcpyAsync(base + tb + xb, first.data(), first.size() * sizeof(int),
+                       cudaMemcpyHostToDevice, ctx->stream));
+    const DevSurf<double>* table = nullptr;
+    rc = upload_table<double>(ctx, surf, S, ctx->stream, &table);
+    if (rc) return rc;
+    jp.table = table;
+    jp.S = S;
+    jp.clip = clip ? 1 : 0;
+    jp.has_rot0 = rot0 != nullptr;
+    if (rot0)
+        for (int i = 0; i < 9; ++i) jp.rot0[i] = rot0[i];
+    jp.P = P;
+    jp.N = N;
+    jp.ld = ld;
+    jp.y0 = (const double*)y0;
+    jp.u0 = (const double*)u0;
+    jp.q = (double*)q;
+    jp.J = (double*)J;
+    const size_t smem = (((size_t)S * sizeof(DevSurf<double>) + 127) & ~size_t(127)) + 16;
+    if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
+    auto kern = (flags & RTX_EXACT) ? jac_kernel<true, JAC_PB> : jac_kernel<false, JAC_PB>;
+    if (smem > 48 * 1024)
+        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const dim3 grid((unsigned)((N + JAC_THREADS - 1) / JAC_THREADS), (unsigned)nblk);
+    return timed(ctx, [&] {
+        kern<<<grid, JAC_THREADS, smem, ctx->stream>>>(jp);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+}
+
+int rtx_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void* J, int64_t ld,
+                      const double* center, double* out) {
+    if (!ctx || !out || N < 0 || (N > 0 && (!q || !J))) return RTX_E_BADARG;
+    if (P < 1 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
+    const int W = 5 + 3 * P + P * (P + 1) / 2;
+    const long long slots = (N + RTX_JAC_SLOT - 1) / RTX_JAC_SLOT;
+    if (slots == 0) {
+        memset(out, 0, (size_t)W * sizeof(double));
+        return 0;
+    }
+    CK(cudaSetDevice(ctx->device));
+    Workspace& ws = ctx->ws[WS_JSUM];
+    const size_t per = (size_t)W * sizeof(double);
+    if ((unsigned long long)slots >= SIZE_MAX / per - 1) return RTX_E_NOMEM;
+    int rc = reserve(ws, (size_t)(slots + 1) * per);
+    if (rc) return rc;
+    double* part = (double*)ws.p;
+    double* sums = part + slots * W;
+    const double cx = center ? center[0] : 0.0, cy = center ? center[1] : 0.0;
+    rc = timed(ctx, [&] {
+        const dim3 grid((unsigned)slots, (unsigned)((W + JSUM_OUT * 256 - 1) / (JSUM_OUT * 256)));
+        jac_sums_kernel<<<grid, 256, 0, ctx->stream>>>((const double*)q, (const double*)J, N, ld,
+                                                        P, cx, cy, W, part);
+        ctx->launches++;
+        int rc = (int)cudaGetLastError();
+        if (rc) return rc;
+        // the slots in slot order: the same second pass as the OTF sums
+        otf_sum_kernel<<<(W + 255) / 256, 256, 0, ctx->stream>>>(part, W, slots, sums);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(out, sums, per, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
 }
 
 }  // extern "C"

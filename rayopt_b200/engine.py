@@ -54,6 +54,7 @@ def spot_spec(z, bins, range, center, radial=False, offsets=None):
 # mirrors `struct rtx_otf` (include/rtx.h)
 OTF_MAX_PLANES, OTF_MAX_FREQS = 16, 256
 OTF_SLOT, OTF_BLOCK = 16384, 16      # RTX_OTF_SLOT, RTX_OTF_BLOCK
+MAX_PARAMS, JAC_SLOT = 64, 16384     # RTX_MAX_PARAMS, RTX_JAC_SLOT
 OTF_DTYPE = np.dtype([("planes", "<i4"), ("nfreq", "<i4"), ("dnu", "<f8"), ("c", "<f8", (2,)),
                       ("z", "<f8", (OTF_MAX_PLANES,)), ("o", "<f8", (OTF_MAX_PLANES, 2))],
                      align=True)
@@ -91,6 +92,18 @@ def otf_bound(spec, N, count, phi, chunks=1):
     slots = -(-int(N)//OTF_SLOT)
     D = OTF_SLOT//8 + 8 + slots + chunks - 1
     return (D + 13*np.asarray(phi, np.float64) + 5*OTF_BLOCK)*2.**-52*np.asarray(count)
+
+
+def jacobian_sums_unpack(out, P):
+    """rtx_jacobian_sums' row (include/rtx.h) as a dict; rows of several
+    calls may be added first"""
+    out = np.asarray(out, np.float64)
+    K = np.zeros((P, P))
+    iu = np.triu_indices(P)
+    K[iu] = out[4 + 3*P:4 + 3*P + len(iu[0])]
+    K.T[iu] = K[iu]
+    return dict(n=out[0], sum_d=out[1:3].copy(), sum_d2=out[3], G=out[4:4 + 2*P].reshape(P, 2),
+                H=out[4 + 2*P:4 + 3*P].copy(), K=K, bad=out[-1], out=out)
 
 
 def spot_shape(spec):
@@ -735,6 +748,60 @@ class Engine:
         check(self.lib.rtx_otf_rows(self.ctx, _code(y.dtype), N, y.ptr, inc.ptr, ptr(spec),
                                     ptr(sums), ptr(count)))
         return sums[..., 0] + 1j*sums[..., 1], count
+
+    # ---- lens-parameter derivatives --------------------------------------
+    def trace_jacobian(self, table, y0, u0, moves, clip=False, rot0=None, exact=False, N=None):
+        """rtx_trace_jacobian: the image point q of every DEVICE launch ray at
+        the last surface of `table` and its derivatives with respect to P
+        parameters.  `moves`: P lists of (row, record), each record the
+        derivative of table[row] (tolerance.record_tangents of this 1-D
+        table, or one wavelength's records of a (W, S) table's).  Returns (q
+        (N, 2), J (P, 2, ld)) DeviceArrays, ld = N rounded up to 32 rays;
+        asynchronous.  q is the last row trace_device stores, bit for bit."""
+        args = self._march(table, y0, u0, N, clip, rot0)
+        N = args[5]
+        if np.dtype(y0.dtype) != np.float64:
+            raise ValueError("the Jacobian is FP64 only, got %s rays" % np.dtype(y0.dtype))
+        P = len(moves)
+        if not 1 <= P <= MAX_PARAMS:
+            raise ValueError("need 1..%d parameters, got %d" % (MAX_PARAMS, P))
+        rows, recs = [], []
+        for p, mv in enumerate(moves):
+            if not len(mv):
+                raise ValueError("parameter %d has no moves" % p)
+            for row, rec in mv:
+                if not 0 <= int(row) < args[2]:
+                    raise ValueError("move row %r is not in 0..%d" % (row, args[2] - 1))
+                rows.append(int(row))
+                recs.append(rec)
+        first = np.cumsum([0] + [len(mv) for mv in moves]).astype(np.int32)
+        rows = np.ascontiguousarray(rows, np.int32)
+        recs = np.ascontiguousarray(np.array(recs, SURFACE_DTYPE))
+        if recs.shape != rows.shape:
+            raise ValueError("each move must be one record (a (W, S) table's record_tangents "
+                             "gives (W,) records: pick one wavelength), got %s for %d moves"
+                             % (recs.shape, len(rows)))
+        ld = max(32, -(-N//32)*32)
+        q, J = self.empty((N, 2)), self.empty((P, 2, ld))
+        check(self.lib.rtx_trace_jacobian(*args, P, ptr(first), ptr(rows), ptr(recs), q.ptr,
+                                          J.ptr, ld, self._flags(exact, False)))
+        return q, J
+
+    def jacobian_sums(self, q, J, center=None, N=None):
+        """rtx_jacobian_sums of trace_jacobian's DEVICE q (N, 2) and J (P, 2,
+        ld) about `center` (2,): a dict of n, sum_d (2,), sum_d2, G (P, 2),
+        H (P,), K (P, P) (symmetric), bad (rays with a finite q and a
+        non-finite derivative) and the raw output row `out`."""
+        P, _, ld = J.shape
+        N = q.shape[0] if N is None else int(N)
+        _check_operands(q.dtype, N, q=(q, 2))
+        if np.dtype(J.dtype) != np.float64 or N > ld:
+            raise ValueError("J must be float64 (P, 2, ld) with ld >= N")
+        c = None if center is None else np.ascontiguousarray(center, np.float64).reshape(2)
+        W = 5 + 3*P + P*(P + 1)//2
+        out = np.zeros(W)
+        check(self.lib.rtx_jacobian_sums(self.ctx, N, P, q.ptr, J.ptr, ld, ptr(c), ptr(out)))
+        return jacobian_sums_unpack(out, P)
 
     def ipc_export(self, darray):
         h = (C.c_ubyte*64)()

@@ -63,6 +63,32 @@ def _parse(params, S):
     return out
 
 
+def _checked(tables, params):
+    """(tables as (W, S) records, params parsed) after every refusal
+    perturbed_tables and record_tangents share (ValueError)"""
+    tables = np.asarray(tables, SURFACE_DTYPE)
+    if tables.ndim == 1:
+        tables = tables[None]
+    S = tables.shape[1]
+    params = _parse(params, S)
+    for j, kind in params:
+        r = tables[:, j - 1]
+        if kind == "distance" and np.any(r["offset"][:, :2] != 0):
+            raise ValueError("surface %d is not on the axis of its predecessor" % j)
+        if kind in ("tilt_x", "tilt_y") and np.any(r["flags"] & F_ROTATED):
+            raise ValueError("surface %d is already rotated" % j)
+        if kind == "index":
+            if j == S:
+                raise ValueError("surface %d is the last: no medium follows it" % j)
+            for rr in (r, tables[:, j]):
+                if np.any(rr["mu"] == -1):
+                    raise ValueError("index of surface %d: a mirror bounds the medium" % j)
+                if np.any((rr["mu"] == 1) & (rr["n"] == rr["n0"])):
+                    raise ValueError("index of surface %d: the medium after it is not "
+                                     "bounded by two materials" % j)
+    return tables, params
+
+
 def _move_distance(off_z, d):
     """rayopt's ``distance += d`` on the offset's z (the element's length
     along its direction, +z or, for a negative distance, -z)"""
@@ -90,29 +116,10 @@ def perturbed_tables(tables, params, deltas):
                medium (mu = 1 and n = n0) on either side
 
     Raises ValueError before building anything."""
-    tables = np.asarray(tables, SURFACE_DTYPE)
-    if tables.ndim == 1:
-        tables = tables[None]
-    W, S = tables.shape
-    params = _parse(params, S)
+    tables, params = _checked(tables, params)
     deltas = np.asarray(deltas, np.float64)
     if deltas.ndim != 2 or deltas.shape[1] != len(params):
         raise ValueError("deltas must be (V, %d), got %s" % (len(params), deltas.shape))
-    for j, kind in params:
-        r = tables[:, j - 1]
-        if kind == "distance" and np.any(r["offset"][:, :2] != 0):
-            raise ValueError("surface %d is not on the axis of its predecessor" % j)
-        if kind in ("tilt_x", "tilt_y") and np.any(r["flags"] & F_ROTATED):
-            raise ValueError("surface %d is already rotated" % j)
-        if kind == "index":
-            if j == S:
-                raise ValueError("surface %d is the last: no medium follows it" % j)
-            for rr in (r, tables[:, j]):
-                if np.any(rr["mu"] == -1):
-                    raise ValueError("index of surface %d: a mirror bounds the medium" % j)
-                if np.any((rr["mu"] == 1) & (rr["n"] == rr["n0"])):
-                    raise ValueError("index of surface %d: the medium after it is not "
-                                     "bounded by two materials" % j)
     V = deltas.shape[0]
     out = np.repeat(tables[None], V, axis=0)
     kc2_rows, mu_rows, angles = set(), set(), {}
@@ -152,6 +159,66 @@ def perturbed_tables(tables, params, deltas):
                 continue
             out["rot"][v, :, r] = _rot_rxyz([float(x) for x in a[v]]).reshape(9)
             out["flags"][v, :, r] |= F_ROTATED
+    return out
+
+
+# d rot_normal / d angle of _rot_rxyz at zero angles, for the angles tilt_x
+# (a[0]) and tilt_y (a[1]) move
+_ROT_GENERATOR = {"tilt_x": np.array([[0., 0., 0.], [0., 0., -1.], [0., 1., 0.]]),
+                  "tilt_y": np.array([[0., 0., 1.], [0., 0., 0.], [-1., 0., 0.]])}
+
+
+def record_tangents(tables, params):
+    """The derivative of perturbed_tables(tables, params, deltas) with
+    respect to each delta at deltas = 0, with the same refusals: a list of P
+    parameters, each a list of moves (row, records), `records` the (W,)
+    derivatives of tables[:, row] (SURFACE_DTYPE; a single record for a 1-D
+    table).  Only the fields perturbed_tables moves are non-zero:
+
+    kind       fields of row j-1 (index: and of row j)
+    curvature  c = 1, kc2 = (1 + k) 2c
+    conic      k = 1, kc2 = c^2
+    distance   offset z = +-1, the sign of _move_distance
+    asph<i>    asph[i] = 1, dasph[i] = 2(i + 1)
+    tilt_x/_y  rot = the generator of _rot_rxyz at zero angles
+    index      row j-1: n = 1, mu = -mu/n, muf = sgn dmu, mu2m1 = 2 mu dmu;
+               row j: n0 = 1, mu = 1/n, muf = sgn dmu, mu2m1 = 2 mu dmu
+
+    Moves are the unit the device Jacobian takes (Engine.trace_jacobian), so
+    a caller may build its own: [(j, d_dist_j), (j + 1, -d_dist_{j+1})]
+    shifts a group of surfaces."""
+    one = np.asarray(tables).ndim == 1
+    tables, params = _checked(tables, params)
+    out = []
+    for j, kind in params:
+        r = j - 1
+        t = tables[:, r]
+        rec = np.zeros(t.shape, SURFACE_DTYPE)
+        moves = [(r, rec)]
+        if kind == "curvature":
+            rec["c"] = 1
+            rec["kc2"] = (1 + t["k"])*2*t["c"]
+        elif kind == "conic":
+            rec["k"] = 1
+            rec["kc2"] = t["c"]**2
+        elif kind.startswith("asph"):
+            i = int(kind[4:])
+            rec["asph"][:, i] = 1
+            rec["dasph"][:, i] = 2*(i + 1)
+        elif kind == "distance":
+            rec["offset"][:, 2] = np.where(np.signbit(t["offset"][:, 2]), -1., 1.)
+        elif kind in ("tilt_x", "tilt_y"):
+            rec["rot"] = _ROT_GENERATOR[kind].reshape(9)
+        else:                                                  # index
+            rec2 = np.zeros(t.shape, SURFACE_DTYPE)
+            moves.append((r + 1, rec2))
+            for x, row, dn, dn0 in ((rec, t, 1., 0.), (rec2, tables[:, r + 1], 0., 1.)):
+                mu, n = row["mu"], row["n"]
+                dmu = (dn0 - mu*dn)/n                          # d(n0/n)
+                x["n"], x["n0"], x["mu"] = dn, dn0, dmu
+                x["muf"] = np.sign(mu)*dmu
+                x["mu2m1"] = 2*mu*dmu
+        out.append([(row, x[0] if one else x) for row, x in moves])
     return out
 
 
