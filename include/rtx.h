@@ -647,6 +647,76 @@ int rtx_trace_jacobian(rtx_ctx *ctx, const rtx_surface *surf, int S,
 int rtx_jacobian_sums(rtx_ctx *ctx, int64_t N, int P, const void *q, const void *J,
                       int64_t ld, const double *center, double *out);
 
+/* ---- lens-parameter derivatives of the wavefront ------------------------ */
+/*
+ * rtx_trace_opd's optical path A of every ray and its exact derivatives
+ * dA = dA/dp with respect to P lens parameters, from one march (forward-mode
+ * tangents; FP64 only).  surf, S, rot0, y0, u0, N, clip and opd are
+ * rtx_trace_opd's (surf = system[1:after+1]); P, param_first, move_row and
+ * moves are rtx_trace_jacobian's, on those rows.  The epilogue's reference
+ * sphere moves with the lens through
+ *  dopd   host, (P, 4) doubles: per parameter d(opd->d)[0..2], d(opd->n_after)
+ * (moves of the image surface reach A only through them); its radius and the
+ * frame change M are held fixed.
+ *  A      DEVICE (N,) doubles
+ *  dA     DEVICE (P, ld) doubles: dA[p ld + k] = dA_k/dp; ld >= N; columns
+ *         N .. ld-1 are not written
+ *
+ * A equals rtx_trace_opd's A for the same arguments, bit for bit, in each
+ * mode (RTX_EXACT or not).  dA is the derivative of that march and
+ * epilogue: the path's tangent adds n0 ds + s dn0 at every surface (s the
+ * surface's intercept distance, n0 its index), the sphere intercept ti is
+ * differentiated implicitly at its root as the surfaces' intercepts are
+ * (rtx_trace_jacobian), and dA = dT + n_after dti + ti d(n_after).  The
+ * input-plane term of an object at infinity has no derivative (the launch
+ * rays are fixed).  The tangents are FP64 with fused multiply-adds in both
+ * modes.  A ray whose A is NaN has NaN derivatives; a finite A may have a
+ * non-finite derivative where the ray grazes a surface (rtx_wavefront_sums
+ * counts those).
+ *
+ * RTX_E_BADARG, before any device work or allocation: every refusal of
+ * rtx_trace_jacobian (with A, dA in place of q, J); a NULL opd, or a NULL
+ * dopd with P > 0; an opd radius that is 0 or not finite; a non-finite dopd
+ * entry; a move with a non-zero rot on row S-1 (M is held fixed).  A record
+ * of surf with n_asph > RTX_MAX_ASPH gives RTX_E_UNSUPPORTED.  The tangent
+ * records and dopd are kept in the context.  Asynchronous;
+ * rtx_last_kernel_ms covers the kernel.
+ */
+int rtx_trace_opd_jacobian(rtx_ctx *ctx, const rtx_surface *surf, int S,
+                           const double *rot0, int dtype, int64_t N, const void *y0,
+                           const void *u0, int clip, const rtx_opd *opd, int P,
+                           const int32_t *param_first, const int32_t *move_row,
+                           const rtx_surface *moves, const double *dopd, void *A,
+                           void *dA, int64_t ld, unsigned flags);
+
+/*
+ * Gauss-Newton sums of rtx_trace_opd_jacobian's A (DEVICE (N,)) and dA
+ * (DEVICE (P, ld)) about the guess piston a0, with d = fl(A - a0).  A ray
+ * enters iff A and all of its P derivatives are finite.  P = 0 is allowed
+ * (dA is then not read and may be NULL): n, sum d and sum d^2 of any A.
+ * out (host, W = 4 + 2P + P(P+1)/2 doubles), over the rays that enter:
+ *   out[0]              n
+ *   out[1]              sum d
+ *   out[2]              sum d^2
+ *   out[3 + a]          G_a = sum dA/dp_a           (a < P)
+ *   out[3 + P + a]      H_a = sum d dA/dp_a
+ *   out[3 + 2P + ...]   K_ab = sum dA/dp_a dA/dp_b, a <= b, row-major
+ *                       packed upper triangle (P(P+1)/2 values)
+ *   out[W - 1]          rays with a finite A and a non-finite derivative
+ *                       (they do not enter)
+ * Deterministic, in the same slots and order as rtx_jacobian_sums, and
+ * within the same bound:
+ *   |out - exact| <= (2 RTX_JAC_SLOT + ceil(N / RTX_JAC_SLOT)) eps sum|term|
+ * where the terms are the single products of d and dA entries each output
+ * adds.  Counts are exact.  RTX_E_BADARG, before any device work or
+ * allocation: NULL ctx or out; NULL A with N > 0, or NULL dA with N > 0 and
+ * P > 0; N < 0; P outside 0..RTX_MAX_PARAMS; ld < N.  The slot sums are kept
+ * in the context: RTX_E_NOMEM before allocating when they do not fit.
+ * Synchronous; rtx_last_kernel_ms covers both kernels.
+ */
+int rtx_wavefront_sums(rtx_ctx *ctx, int64_t N, int P, const void *A, const void *dA,
+                       int64_t ld, double a0, double *out);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

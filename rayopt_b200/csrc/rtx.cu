@@ -2030,7 +2030,7 @@ void add_tangent(const rtx_surface& s, JacTan& d) {
     d.c += s.c;
     d.k1 += s.k;
     d.kc2 += s.kc2;
-    d.mu += s.mu;
+    d.n0 += s.n0;
     d.muf += s.muf;
     d.mu2m1 += s.mu2m1;
     for (int i = 0; i < RTX_MAX_ASPH; ++i) {
@@ -2039,15 +2039,15 @@ void add_tangent(const rtx_surface& s, JacTan& d) {
         if (d.asph[i] != 0.0 || d.dasph[i] != 0.0) d.n_asph = std::max(d.n_asph, i + 1);
     }
 }
-}  // namespace
 
-extern "C" {
-
-int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
-                       int dtype, int64_t N, const void* y0, const void* u0, int clip, int P,
-                       const int32_t* param_first, const int32_t* move_row,
-                       const rtx_surface* moves, void* q, void* J, int64_t ld, unsigned flags) {
-    if (!ctx || !param_first || !move_row || !moves || !q || !J) return RTX_E_BADARG;
+// rtx_trace_jacobian (dopd NULL: jp holds q, J) and rtx_trace_opd_jacobian
+// (jp holds the rtx_opd members, A, dA): the refusals they share, the
+// tangent records and the launch
+int jacobian_march(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0, int dtype,
+                   int64_t N, const void* y0, const void* u0, int clip, int P,
+                   const int32_t* param_first, const int32_t* move_row, const rtx_surface* moves,
+                   const double* dopd, int64_t ld, unsigned flags, JacParams& jp) {
+    if (!ctx || !param_first || !move_row || !moves) return RTX_E_BADARG;
     if (!surf || S < 1 || S > RTX_MAX_SURFACES || N < 0 || !y0 || !u0) return RTX_E_BADARG;
     if (dtype != RTX_F64 || P < 1 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
     if (param_first[0] != 0) return RTX_E_BADARG;
@@ -2061,12 +2061,24 @@ int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const doubl
         if (surf[move_row[m]].mu == 1.0 && (mv.mu != 0.0 || mv.muf != 0.0 || mv.mu2m1 != 0.0))
             return RTX_E_BADARG;
     }
+    const bool opd = dopd != nullptr;
+    if (opd) {  // rtx_trace_opd_jacobian: P, param_first and move_row are checked above
+        for (int i = 0; i < 4 * P; ++i)
+            if (!std::isfinite(dopd[i])) return RTX_E_BADARG;
+        // the frame change M to the image surface is held fixed: no tilt of
+        // surface S-1 (`after`)
+        for (int m = 0; m < param_first[P]; ++m)
+            if (move_row[m] == S - 1)
+                for (int i = 0; i < 9; ++i)
+                    if (moves[m].rot[i] != 0.0) return RTX_E_BADARG;
+    }
     int rc = check_table(surf, S);
     if (rc) return rc;
     if (N == 0) return 0;
+    const int PB = opd ? JAC_OPD_PB : JAC_PB;
     // the tangent records: one per (parameter, moved row), their (P, S) index
-    // and the first moved row of each block of JAC_PB parameters
-    const int nblk = (P + JAC_PB - 1) / JAC_PB;
+    // and the first moved row of each block of PB parameters
+    const int nblk = (P + PB - 1) / PB;
     std::vector<int> idx((size_t)P * S, -1), first(nblk, S);
     std::vector<JacTan> tan;
     for (int p = 0; p < P; ++p)
@@ -2078,17 +2090,16 @@ int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const doubl
                 memset(&tan.back(), 0, sizeof(JacTan));
             }
             add_tangent(moves[m], tan[(size_t)k]);
-            first[p / JAC_PB] = std::min(first[p / JAC_PB], (int)move_row[m]);
+            first[p / PB] = std::min(first[p / PB], (int)move_row[m]);
         }
     auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t tb = up(tan.size() * sizeof(JacTan)), xb = up(idx.size() * sizeof(int));
+    const size_t fb = up(first.size() * sizeof(int)), db = opd ? (size_t)P * 4 * sizeof(double) : 0;
     CK(cudaSetDevice(ctx->device));
     Workspace& ws = ctx->ws[WS_JAC];
-    rc = reserve(ws, tb + xb + first.size() * sizeof(int));
+    rc = reserve(ws, tb + xb + fb + db);
     if (rc) return rc;
     unsigned char* base = (unsigned char*)ws.p;
-    JacParams jp;
-    memset(&jp, 0, sizeof(jp));
     jp.tan = (const JacTan*)base;
     jp.idx = (const int*)(base + tb);
     jp.first = (const int*)(base + tb + xb);
@@ -2099,6 +2110,10 @@ int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const doubl
                        ctx->stream));
     CK(cudaMemcpyAsync(base + tb + xb, first.data(), first.size() * sizeof(int),
                        cudaMemcpyHostToDevice, ctx->stream));
+    if (opd) {
+        jp.dopd = (const double*)(base + tb + xb + fb);
+        CK(cudaMemcpyAsync(base + tb + xb + fb, dopd, db, cudaMemcpyHostToDevice, ctx->stream));
+    }
     const DevSurf<double>* table = nullptr;
     rc = upload_table<double>(ctx, surf, S, ctx->stream, &table);
     if (rc) return rc;
@@ -2113,11 +2128,11 @@ int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const doubl
     jp.ld = ld;
     jp.y0 = (const double*)y0;
     jp.u0 = (const double*)u0;
-    jp.q = (double*)q;
-    jp.J = (double*)J;
     const size_t smem = (((size_t)S * sizeof(DevSurf<double>) + 127) & ~size_t(127)) + 16;
     if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
-    auto kern = (flags & RTX_EXACT) ? jac_kernel<true, JAC_PB> : jac_kernel<false, JAC_PB>;
+    const bool exact = flags & RTX_EXACT;
+    auto kern = opd ? (exact ? jac_kernel<true, JAC_OPD_PB, true> : jac_kernel<false, JAC_OPD_PB, true>)
+                    : (exact ? jac_kernel<true, JAC_PB, false> : jac_kernel<false, JAC_PB, false>);
     if (smem > 48 * 1024)
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const dim3 grid((unsigned)((N + JAC_THREADS - 1) / JAC_THREADS), (unsigned)nblk);
@@ -2128,11 +2143,11 @@ int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const doubl
     });
 }
 
-int rtx_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void* J, int64_t ld,
-                      const double* center, double* out) {
-    if (!ctx || !out || N < 0 || (N > 0 && (!q || !J))) return RTX_E_BADARG;
-    if (P < 1 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
-    const int W = 5 + 3 * P + P * (P + 1) / 2;
+// rtx_jacobian_sums (NC = 2) and rtx_wavefront_sums (NC = 1): W outputs of
+// the slot sums, then the slots in slot order
+template <int NC>
+int gauss_newton_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void* J, int64_t ld,
+                      double c0, double c1, int W, double* out) {
     const long long slots = (N + RTX_JAC_SLOT - 1) / RTX_JAC_SLOT;
     if (slots == 0) {
         memset(out, 0, (size_t)W * sizeof(double));
@@ -2146,11 +2161,10 @@ int rtx_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void*
     if (rc) return rc;
     double* part = (double*)ws.p;
     double* sums = part + slots * W;
-    const double cx = center ? center[0] : 0.0, cy = center ? center[1] : 0.0;
     rc = timed(ctx, [&] {
         const dim3 grid((unsigned)slots, (unsigned)((W + JSUM_OUT * 256 - 1) / (JSUM_OUT * 256)));
-        jac_sums_kernel<<<grid, 256, 0, ctx->stream>>>((const double*)q, (const double*)J, N, ld,
-                                                        P, cx, cy, W, part);
+        jac_sums_kernel<NC><<<grid, 256, 0, ctx->stream>>>((const double*)q, (const double*)J, N,
+                                                            ld, P, c0, c1, W, part);
         ctx->launches++;
         int rc = (int)cudaGetLastError();
         if (rc) return rc;
@@ -2163,6 +2177,62 @@ int rtx_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void*
     CK(cudaMemcpyAsync(out, sums, per, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
+                       int dtype, int64_t N, const void* y0, const void* u0, int clip, int P,
+                       const int32_t* param_first, const int32_t* move_row,
+                       const rtx_surface* moves, void* q, void* J, int64_t ld, unsigned flags) {
+    if (!q || !J) return RTX_E_BADARG;
+    JacParams jp;
+    memset(&jp, 0, sizeof(jp));
+    jp.q = (double*)q;
+    jp.J = (double*)J;
+    return jacobian_march(ctx, surf, S, rot0, dtype, N, y0, u0, clip, P, param_first, move_row,
+                          moves, nullptr, ld, flags, jp);
+}
+
+int rtx_trace_opd_jacobian(rtx_ctx* ctx, const rtx_surface* surf, int S, const double* rot0,
+                           int dtype, int64_t N, const void* y0, const void* u0, int clip,
+                           const rtx_opd* opd, int P, const int32_t* param_first,
+                           const int32_t* move_row, const rtx_surface* moves, const double* dopd,
+                           void* A, void* dA, int64_t ld, unsigned flags) {
+    if (!opd || !A || !dA || (P > 0 && !dopd)) return RTX_E_BADARG;
+    if (opd->radius == 0.0 || !std::isfinite(opd->radius)) return RTX_E_BADARG;
+    JacParams jp;
+    memset(&jp, 0, sizeof(jp));
+    jp.infinite = opd->infinite;
+    for (int k = 0; k < 3; ++k) {
+        jp.y0r[k] = opd->y0_ref[k];
+        jp.u0r[k] = opd->u0_ref[k];
+        jp.d[k] = opd->d[k];
+    }
+    for (int k = 0; k < 9; ++k) jp.M[k] = opd->M[k];
+    jp.n0 = opd->n0;
+    jp.n_after = opd->n_after;
+    jp.radius = opd->radius;
+    jp.A = (double*)A;
+    jp.dA = (double*)dA;
+    return jacobian_march(ctx, surf, S, rot0, dtype, N, y0, u0, clip, P, param_first, move_row,
+                          moves, dopd, ld, flags, jp);
+}
+
+int rtx_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, const void* J, int64_t ld,
+                      const double* center, double* out) {
+    if (!ctx || !out || N < 0 || (N > 0 && (!q || !J))) return RTX_E_BADARG;
+    if (P < 1 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
+    return gauss_newton_sums<2>(ctx, N, P, q, J, ld, center ? center[0] : 0.0,
+                                center ? center[1] : 0.0, 5 + 3 * P + P * (P + 1) / 2, out);
+}
+
+int rtx_wavefront_sums(rtx_ctx* ctx, int64_t N, int P, const void* A, const void* dA, int64_t ld,
+                       double a0, double* out) {
+    if (!ctx || !out || N < 0 || (N > 0 && (!A || (P > 0 && !dA)))) return RTX_E_BADARG;
+    if (P < 0 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
+    return gauss_newton_sums<1>(ctx, N, P, A, dA, ld, a0, 0.0, 4 + 2 * P + P * (P + 1) / 2, out);
 }
 
 }  // extern "C"

@@ -106,6 +106,18 @@ def jacobian_sums_unpack(out, P):
                 H=out[4 + 2*P:4 + 3*P].copy(), K=K, bad=out[-1], out=out)
 
 
+def wavefront_sums_unpack(out, P):
+    """rtx_wavefront_sums' row (include/rtx.h) as a dict; rows of several
+    calls may be added first"""
+    out = np.asarray(out, np.float64)
+    K = np.zeros((P, P))
+    iu = np.triu_indices(P)
+    K[iu] = out[3 + 2*P:3 + 2*P + len(iu[0])]
+    K.T[iu] = K[iu]
+    return dict(n=out[0], sum_d=out[1], sum_d2=out[2], G=out[3:3 + P].copy(),
+                H=out[3 + P:3 + 2*P].copy(), K=K, bad=out[-1], out=out)
+
+
 def spot_shape(spec):
     """(K, nx, ny) of a 2-D record, (K, nx) of a radial one"""
     s = spec[0]
@@ -167,6 +179,46 @@ def _check_trace_operands(dtype, N, rows, ld, outputs, mask=None, path_sum=None)
 def _rot0(rot0):
     """the optional 3x3 launch rotation as 9 contiguous doubles"""
     return None if rot0 is None else np.ascontiguousarray(rot0, np.float64).reshape(9)
+
+
+def _opd_record(spec):
+    """the rtx_opd record of a dict with its members (lazy.opd_spec)"""
+    rec = np.zeros(1, OPD_DTYPE)
+    for k in ("y0_ref", "u0_ref", "M", "d"):
+        rec[k] = np.asarray(spec[k], float).reshape(rec[k].shape[1:])
+    for k in ("n0", "n_after", "radius"):
+        rec[k] = float(spec[k])
+    rec["infinite"] = int(bool(spec["infinite"]))
+    return rec
+
+
+def _moves(y0, moves, S):
+    """(P, param_first, move_row, moves) of the derivative marches from P
+    lists of (row, record) on a table of S rows; ValueError for FP32 rays,
+    a bad P, a parameter without moves, a row out of range or a move that
+    is not one record"""
+    if np.dtype(y0.dtype) != np.float64:
+        raise ValueError("the Jacobian is FP64 only, got %s rays" % np.dtype(y0.dtype))
+    P = len(moves)
+    if not 1 <= P <= MAX_PARAMS:
+        raise ValueError("need 1..%d parameters, got %d" % (MAX_PARAMS, P))
+    rows, recs = [], []
+    for p, mv in enumerate(moves):
+        if not len(mv):
+            raise ValueError("parameter %d has no moves" % p)
+        for row, rec in mv:
+            if not 0 <= int(row) < S:
+                raise ValueError("move row %r is not in 0..%d" % (row, S - 1))
+            rows.append(int(row))
+            recs.append(rec)
+    first = np.cumsum([0] + [len(mv) for mv in moves]).astype(np.int32)
+    rows = np.ascontiguousarray(rows, np.int32)
+    recs = np.ascontiguousarray(np.array(recs, SURFACE_DTYPE))
+    if recs.shape != rows.shape:
+        raise ValueError("each move must be one record (a (W, S) table's record_tangents "
+                         "gives (W,) records: pick one wavelength), got %s for %d moves"
+                         % (recs.shape, len(rows)))
+    return P, first, rows, recs
 
 
 def _given(yp):
@@ -683,13 +735,8 @@ class Engine:
         """rtx_trace_opd: `spec` a dict with the members of `struct rtx_opd`
         (include/rtx.h); A (N,), P (N,3) DeviceArrays.  Asynchronous."""
         args = self._march(table, y0, u0, N, clip, rot0, A=(A, 1), P=(P, 3))
-        rec = np.zeros(1, OPD_DTYPE)
-        for k in ("y0_ref", "u0_ref", "M", "d"):
-            rec[k] = np.asarray(spec[k], float).reshape(rec[k].shape[1:])
-        for k in ("n0", "n_after", "radius"):
-            rec[k] = float(spec[k])
-        rec["infinite"] = int(bool(spec["infinite"]))
-        check(self.lib.rtx_trace_opd(*args, ptr(rec), A.ptr, P.ptr, self._flags(exact, False)))
+        check(self.lib.rtx_trace_opd(*args, ptr(_opd_record(spec)), A.ptr, P.ptr,
+                                     self._flags(exact, False)))
 
     @staticmethod
     def _spot_outputs(spec, counts, extent):
@@ -760,27 +807,7 @@ class Engine:
         asynchronous.  q is the last row trace_device stores, bit for bit."""
         args = self._march(table, y0, u0, N, clip, rot0)
         N = args[5]
-        if np.dtype(y0.dtype) != np.float64:
-            raise ValueError("the Jacobian is FP64 only, got %s rays" % np.dtype(y0.dtype))
-        P = len(moves)
-        if not 1 <= P <= MAX_PARAMS:
-            raise ValueError("need 1..%d parameters, got %d" % (MAX_PARAMS, P))
-        rows, recs = [], []
-        for p, mv in enumerate(moves):
-            if not len(mv):
-                raise ValueError("parameter %d has no moves" % p)
-            for row, rec in mv:
-                if not 0 <= int(row) < args[2]:
-                    raise ValueError("move row %r is not in 0..%d" % (row, args[2] - 1))
-                rows.append(int(row))
-                recs.append(rec)
-        first = np.cumsum([0] + [len(mv) for mv in moves]).astype(np.int32)
-        rows = np.ascontiguousarray(rows, np.int32)
-        recs = np.ascontiguousarray(np.array(recs, SURFACE_DTYPE))
-        if recs.shape != rows.shape:
-            raise ValueError("each move must be one record (a (W, S) table's record_tangents "
-                             "gives (W,) records: pick one wavelength), got %s for %d moves"
-                             % (recs.shape, len(rows)))
+        P, first, rows, recs = _moves(y0, moves, args[2])
         ld = max(32, -(-N//32)*32)
         q, J = self.empty((N, 2)), self.empty((P, 2, ld))
         check(self.lib.rtx_trace_jacobian(*args, P, ptr(first), ptr(rows), ptr(recs), q.ptr,
@@ -802,6 +829,44 @@ class Engine:
         out = np.zeros(W)
         check(self.lib.rtx_jacobian_sums(self.ctx, N, P, q.ptr, J.ptr, ld, ptr(c), ptr(out)))
         return jacobian_sums_unpack(out, P)
+
+    def trace_opd_jacobian(self, table, y0, u0, spec, moves, dopd, clip=False, rot0=None,
+                           exact=False, N=None):
+        """rtx_trace_opd_jacobian: trace_opd's path A of every DEVICE launch
+        ray (`table` = system[1:after+1], `spec` as trace_opd's) and its
+        derivatives with respect to P parameters.  `moves` as
+        trace_jacobian's, on the rows of `table`; `dopd` (P, 4) the
+        derivatives of spec's d and n_after.  Returns (A (N,), dA (P, ld))
+        DeviceArrays, ld = N rounded up to 32 rays; asynchronous.  A is
+        trace_opd's, bit for bit."""
+        args = self._march(table, y0, u0, N, clip, rot0)
+        N = args[5]
+        P, first, rows, recs = _moves(y0, moves, args[2])
+        dopd = np.ascontiguousarray(dopd, np.float64)
+        if dopd.shape != (P, 4):
+            raise ValueError("dopd must be (%d, 4), got %s" % (P, dopd.shape))
+        ld = max(32, -(-N//32)*32)
+        A, dA = self.empty((N,)), self.empty((P, ld))
+        check(self.lib.rtx_trace_opd_jacobian(*args, ptr(_opd_record(spec)), P, ptr(first),
+                                              ptr(rows), ptr(recs), ptr(dopd), A.ptr, dA.ptr, ld,
+                                              self._flags(exact, False)))
+        return A, dA
+
+    def wavefront_sums(self, A, dA, a0=0., N=None):
+        """rtx_wavefront_sums of trace_opd_jacobian's DEVICE A (N,) and dA
+        (P, ld) (None: P = 0, the sums of A alone) about the piston `a0`: a
+        dict of n, sum_d, sum_d2, G (P,), H (P,), K (P, P) (symmetric), bad
+        and the raw output row `out`."""
+        N = A.shape[0] if N is None else int(N)
+        _check_operands(A.dtype, N, A=(A, 1))
+        P, ld = (0, max(N, 1)) if dA is None else dA.shape
+        if np.dtype(A.dtype) != np.float64 or (dA is not None and np.dtype(dA.dtype) != np.float64) \
+                or N > ld:
+            raise ValueError("A must be float64 (N,) and dA float64 (P, ld) with ld >= N")
+        out = np.zeros(4 + 2*P + P*(P + 1)//2)
+        check(self.lib.rtx_wavefront_sums(self.ctx, N, P, A.ptr, None if dA is None else dA.ptr,
+                                          ld, float(a0), ptr(out)))
+        return wavefront_sums_unpack(out, P)
 
     def ipc_export(self, darray):
         h = (C.c_ubyte*64)()

@@ -20,13 +20,28 @@ focus).  Each iteration re-aims the lens, takes the Jacobian, solves
 (J^T J + lambda diag J^T J) delta = -J^T r for a few lambda, scores every
 trial step in one rtx_trace_reduce_many launch on the same bundles and takes
 the best one if it lowers the merit.
+
+``wavefront_jacobian`` and ``optimize_wavefront`` do the same for the rms
+wavefront error, piston removed and referenced to the chief ray: the
+per-ray path A of ``opd()`` (rtx_trace_opd_jacobian, to surface after =
+len(system) - 2, the default reference sphere) in waves W_k = -(A_k -
+A_ref)/lambda.  With d_k = A_k - a0 (a0 the chief ray's A) and the
+one-component sums of rtx_wavefront_sums,
+
+    rms^2 = (sum d^2/n - dbar^2)/lambda^2,   J^T J = (K - G G^T/n)/(n lambda^2),
+    J^T r = (H - dbar G)/(n lambda^2)
+
+The sphere's radius and the frame change to the image surface are held at
+their values for the current lens; its centre, the chief ray's image point,
+moves with the parameters.
 """
 import copy
 
 import numpy as np
 
-from .engine import Engine, default_engine, jacobian_sums_unpack
-from .surface_table import RTX_MAX_ASPH, pack_system
+from .engine import Engine, default_engine, jacobian_sums_unpack, wavefront_sums_unpack
+from .lazy import opd_spec
+from .surface_table import RTX_MAX_ASPH, SURFACE_DTYPE, pack_system
 from .tolerance import _chief, launch_bundles, perturbed_tables, record_tangents
 
 OPT_KINDS = ("curvature", "conic", "distance") + tuple("asph%d" % i for i in range(RTX_MAX_ASPH))
@@ -45,7 +60,9 @@ class _Bundles:
     def __init__(self, system, heights, wavelengths, nrays, distribution, eng, exact):
         self.nominal, self.rot0 = _nominal(system, wavelengths)
         self.W = len(wavelengths)
+        self.wavelengths = list(wavelengths)
         self.rays, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
+        self.chiefs = chiefs
         try:
             self.centers = np.array([_chief(eng, self.nominal[b % self.W], self.rot0, y, u, exact)
                                      for b, (y, u) in enumerate(chiefs)])
@@ -187,6 +204,69 @@ def _merits(eng, B, params, deltas, weights, clip, exact):
     return (weights.reshape(-1)*rms**2).sum(1)
 
 
+def _check_kinds(params):
+    params = [(int(j), kind) for j, kind in params]
+    for j, kind in params:
+        if kind not in OPT_KINDS:
+            raise ValueError("cannot optimise %r: the kinds are %s" % (kind, ", ".join(OPT_KINDS[:4])
+                                                                        + ", asph<i>"))
+    return params
+
+
+def _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
+        distribution, lambdas, eng, exact, prepare, jacobian, merits):
+    """The Levenberg-Marquardt loop of optimize_spot and optimize_wavefront
+    on a copy of `system`.  Per iteration, on the re-aimed bundles B:
+    state = prepare(system, B, final) (freed by state.close() when it has
+    one; `final`: only the merit of the last, re-aimed lens is wanted),
+    jacobian(B, state) the per-bundle normal equations (JtJ (H, W, P, P),
+    Jtr (H, W, P)), merits(B, state, deltas) the weighted merit of each
+    row of deltas on the fixed bundles."""
+    H, W, P = len(heights), len(wavelengths), len(params)
+    weights = np.ones((H, W)) if weights is None else np.broadcast_to(
+        np.asarray(weights, np.float64), (H, W))
+    system = copy.deepcopy(system)
+    total = np.zeros(P)
+    hist = dict(merit=[], lam=[], step=[], trial=[])
+    lam = float(damping)
+    for it in range(iterations + 1):
+        B = _Bundles(system, heights, wavelengths, nrays, distribution, eng, exact)
+        state = None
+        try:
+            state = prepare(system, B, it == iterations)
+            if it == iterations:               # the final lens, re-aimed
+                hist["merit"].append(float(merits(B, state, np.zeros((1, P)), weights)[0]))
+                break
+            res = jacobian(B, state)
+            w = weights[..., None, None]
+            JtJ = (w*res["JtJ"]).sum((0, 1))
+            Jtr = (w[..., 0]*res["Jtr"]).sum((0, 1))
+            lams = [lam*f for f in lambdas]
+            steps = np.array([lm_step(JtJ, Jtr, x) for x in lams])
+            merit = merits(B, state, np.vstack([np.zeros(P), steps]), weights)
+        finally:
+            if state is not None and hasattr(state, "close"):
+                state.close()
+            B.close()
+        hist["merit"].append(float(merit[0]))
+        k = int(np.nanargmin(merit[1:])) if np.isfinite(merit[1:]).any() else -1
+        if k >= 0 and merit[1 + k] < merit[0]:
+            lam = lams[k]
+            apply_deltas(system, params, steps[k])
+            total += steps[k]
+            hist["lam"].append(lam)
+            hist["step"].append(steps[k])
+            hist["trial"].append(float(merit[1 + k]))
+        else:
+            lam *= 100
+            hist["lam"].append(0.)
+            hist["step"].append(np.zeros(P))
+            hist["trial"].append(float(merit[0]))
+    return dict(system=system, deltas=total, merit=np.array(hist["merit"]),
+                lam=np.array(hist["lam"]), step=np.array(hist["step"]).reshape(-1, P),
+                trial=np.array(hist["trial"]), params=params)
+
+
 def optimize_spot(system, params, heights=(0., .707, 1.), wavelengths=None, weights=None,
                   iterations=20, damping=1e-3, nrays=1000, distribution="hexapolar", clip=False,
                   lambdas=(.1, 1., 10., 100.), chunk=1 << 20, engine=None, exact=False):
@@ -206,53 +286,310 @@ def optimize_spot(system, params, heights=(0., .707, 1.), wavelengths=None, weig
     and at the end, lam and step (iterations,) the lambda and step taken (0
     where none was accepted), trial (iterations,) the fixed-bundle merit of
     the accepted step (or of the lens when none was)."""
-    params = [(int(j), kind) for j, kind in params]
-    for j, kind in params:
-        if kind not in OPT_KINDS:
-            raise ValueError("cannot optimise %r: the kinds are %s" % (kind, ", ".join(OPT_KINDS[:4])
-                                                                        + ", asph<i>"))
+    params = _check_kinds(params)
     eng = engine or default_engine()
     wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
     heights = list(heights)
     H, W, P = len(heights), len(wavelengths), len(params)
-    weights = np.ones((H, W)) if weights is None else np.broadcast_to(
-        np.asarray(weights, np.float64), (H, W))
-    system = copy.deepcopy(system)
     record_tangents(_nominal(system, wavelengths)[0], params)  # refusals before any device work
-    total = np.zeros(P)
-    hist = dict(merit=[], lam=[], step=[], trial=[])
-    lam = float(damping)
-    for it in range(iterations + 1):
-        B = _Bundles(system, heights, wavelengths, nrays, distribution, eng, exact)
+
+    def jacobian(B, state):
+        moves = record_tangents(B.nominal, params)
+        return _result(_sums(eng, B, moves, clip, int(chunk), exact), H, W, P, {})
+
+    return _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
+               distribution, lambdas, eng, exact, lambda system, B, final: None, jacobian,
+               lambda B, state, deltas, w: _merits(eng, B, params, deltas, w, clip, exact))
+
+
+# ---- the rms wavefront error ---------------------------------------------
+def _wavefront_checked(system, wavelengths, params):
+    """record_tangents' refusals, then the ones of the wavefront: shape
+    parameters of the image surface (they change only the reference) and
+    tilts of the last two surfaces (they change the frame change M, which is
+    held fixed).  ValueError before any device work."""
+    L = len(system)
+    record_tangents(_nominal(system, wavelengths)[0], params)
+    for j, kind in params:
+        if j == L - 1 and kind not in ("distance",):
+            raise ValueError("%s of the image surface %d changes only the reference sphere"
+                             % (kind, j))
+        if j >= L - 2 and kind in ("tilt_x", "tilt_y"):
+            raise ValueError("%s of surface %d changes the frame change to the image, "
+                             "which the wavefront derivative holds fixed" % (kind, j))
+
+
+def _image_slope(rec, x, y):
+    """e of the normal (x e, y e, 1) of record `rec` at (x, y): the sag's
+    gradient is -(x e, y e)"""
+    r2 = x*x + y*y
+    c, kc2 = float(rec["c"]), float(rec["kc2"])
+    e = -c/np.sqrt(1 - kc2*r2)
+    for j in range(max(int(rec["n_asph"]), 0)):
+        e -= float(rec["dasph"][j])*r2**j
+    return e
+
+
+def _image_sag(rec, x, y):
+    """z of record `rec`'s surface at (x, y)"""
+    r2 = x*x + y*y
+    c, kc2 = float(rec["c"]), float(rec["kc2"])
+    z = c*r2/(1 + np.sqrt(1 - kc2*r2))
+    for j in range(max(int(rec["n_asph"]), 0)):
+        z += float(rec["asph"][j])*r2**(j + 1)
+    return z
+
+
+class _Wavefront:
+    """Per bundle of B: the rtx_opd record of opd()'s default sphere (or of
+    `radius`), its derivative dopd (P, 4), the piston guess a0 (the chief
+    ray's A), the wavelength in lens units and the chief rays on the device.
+    `moves` the full-table moves of record_tangents(B.nominal) (None: no
+    derivatives)."""
+
+    def __init__(self, eng, system, B, heights, moves, radius, clip, exact):
+        L = len(system)
+        self.after, self.image = L - 2, L - 1
+        ei = system[self.image]
+        self.Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else np.eye(3)
+        S = B.nominal.shape[1]
+        self.chief = []
+        self.specs, self.dopd, self.a0, self.wl, self.yimg = [], [], [], [], []
         try:
-            if it == iterations:               # the final lens, re-aimed
-                hist["merit"].append(float(_merits(eng, B, params, np.zeros((1, P)), weights,
-                                                   clip, exact)[0]))
-                break
-            moves = record_tangents(B.nominal, params)
-            res = _result(_sums(eng, B, moves, clip, int(chunk), exact), H, W, P, {})
-            w = weights[..., None, None]
-            JtJ = (w*res["JtJ"]).sum((0, 1))
-            Jtr = (w[..., 0]*res["Jtr"]).sum((0, 1))
-            lams = [lam*f for f in lambdas]
-            steps = np.array([lm_step(JtJ, Jtr, x) for x in lams])
-            merit = _merits(eng, B, params, np.vstack([np.zeros(P), steps]), weights, clip, exact)
+            for b, (y0, u0) in enumerate(B.chiefs):
+                self.chief.append((eng.to_device(np.reshape(y0, (1, 3))),
+                                   eng.to_device(np.reshape(u0, (1, 3)))))
+            for b, (y0, u0) in enumerate(B.chiefs):
+                w = b % B.W
+                table = B.nominal[w]
+                l = B.wavelengths[w]
+                Y = eng.trace(table, np.reshape(y0, (1, 3)), np.reshape(u0, (1, 3)), clip=True,
+                              rot0=B.rot0, keep_last=True, exact=exact, want=("y",))[0][0, 0]
+                if not np.all(np.isfinite(Y)):
+                    raise ValueError("the chief ray of height %g at wavelength %g does not reach "
+                                     "the image" % (heights[b//B.W], l))
+                spec = opd_spec(system, system.track, system.origins, self.after, self.image,
+                                system.refractive_index(l, 0), float(table[S - 2]["n"]),
+                                np.reshape(y0, 3), np.reshape(u0, 3), Y, radius)
+                self.specs.append(spec)
+                self.yimg.append(Y)
+                self.wl.append(l/system.scale)
+                if moves is not None:
+                    self.dopd.append(self._dopd(eng, system, B, b, table, moves, Y, exact))
+                A, Pp = eng.empty((1,)), eng.empty((1, 3))
+                try:
+                    cy, cu = self.chief[b]
+                    eng.trace_opd(table[:-1], cy, cu, spec, A, Pp, clip=clip, rot0=B.rot0,
+                                  exact=exact)
+                    self.a0.append(float(A.download()[0]))
+                finally:
+                    A.free(), Pp.free()
+        except Exception:
+            self.close()
+            raise
+
+    def _dopd(self, eng, system, B, b, table, moves, Y, exact):
+        """d(spec d) and d(n_after) per parameter: the image surface's offset
+        and the chief ray's image point move the sphere's centre"""
+        S = len(table)
+        w = b % B.W
+        mv = [[(row, rec[w]) for row, rec in m] for m in moves]
+        cy, cu = self.chief[b]
+        q, J = eng.trace_jacobian(table, cy, cu, mv, clip=True, rot0=B.rot0, exact=exact)
+        try:
+            dq = J.download()[:, :, 0]
         finally:
-            B.close()
-        hist["merit"].append(float(merit[0]))
-        k = int(np.nanargmin(merit[1:])) if np.isfinite(merit[1:]).any() else -1
-        if k >= 0 and merit[1 + k] < merit[0]:
-            lam = lams[k]
-            apply_deltas(system, params, steps[k])
-            total += steps[k]
-            hist["lam"].append(lam)
-            hist["step"].append(steps[k])
-            hist["trial"].append(float(merit[1 + k]))
-        else:
-            lam *= 100
-            hist["lam"].append(0.)
-            hist["step"].append(np.zeros(P))
-            hist["trial"].append(float(merit[0]))
-    return dict(system=system, deltas=total, merit=np.array(hist["merit"]),
-                lam=np.array(hist["lam"]), step=np.array(hist["step"]).reshape(-1, P),
-                trial=np.array(hist["trial"]), params=params)
+            q.free(), J.free()
+        J = dq
+        Ri = self.Ri
+        e = _image_slope(table[S - 1], Y[0], Y[1])
+        out = np.zeros((len(mv), 4))
+        for p, m in enumerate(mv):
+            dy = np.array([J[p, 0], J[p, 1], -e*(Y[0]*J[p, 0] + Y[1]*J[p, 1])])
+            doff = sum((np.asarray(rec["offset"], float) for row, rec in m if row == S - 1),
+                       np.zeros(3))
+            out[p, :3] = -doff @ Ri.T - dy
+            out[p, 3] = sum(float(rec["n"]) for row, rec in m if row == S - 2)
+        return out
+
+    def close(self):
+        for y, u in self.chief:
+            y.free(), u.free()
+        self.chief = []
+
+
+def _opd_moves(moves, w, S):
+    """the moves of wavelength w on the OPD march's rows 0..S-2; a
+    parameter that moves only the image row gets a zero move on row S-2"""
+    out = []
+    for m in moves:
+        mv = [(row, rec[w]) for row, rec in m if row < S - 1]
+        out.append(mv or [(S - 2, np.zeros((), SURFACE_DTYPE))])
+    return out
+
+
+def _wavefront_sums(eng, B, st, moves, clip, chunk, exact):
+    """(bundles, W) device wavefront sums of every bundle, its ray chunks
+    added on the host in chunk order"""
+    P = len(moves)
+    S = B.nominal.shape[1]
+    out = np.zeros((len(B.rays), 4 + 2*P + P*(P + 1)//2))
+    for b, (y0, u0) in enumerate(B.rays):
+        w = b % B.W
+        mv = _opd_moves(moves, w, S)
+        N = y0.shape[0]
+        for r0 in range(0, N, chunk):
+            r1 = min(N, r0 + chunk)
+            A, dA = eng.trace_opd_jacobian(B.nominal[w, :-1], y0.rows(r0, r1), u0.rows(r0, r1),
+                                           st.specs[b], mv, st.dopd[b], clip=clip, rot0=B.rot0,
+                                           exact=exact)
+            try:
+                out[b] += eng.wavefront_sums(A, dA, st.a0[b])["out"]
+            finally:
+                A.free(), dA.free()
+    return out
+
+
+def gauss_newton_wavefront(out, P, wl):
+    """rms^2 in waves^2 about the mean, J^T J, J^T r and the gradient of
+    rms^2 of one bundle from its rtx_wavefront_sums row `out` and the
+    wavelength wl in lens units (the module docstring's formulas)"""
+    s = wavefront_sums_unpack(out, P)
+    n, G = s["n"], s["G"]
+    k = 1/(wl*wl)
+    with np.errstate(all="ignore"):
+        dbar = s["sum_d"]/n
+        rms2 = (s["sum_d2"]/n - dbar*dbar)*k
+        JtJ = (s["K"] - np.outer(G, G)/n)/n*k
+        Jtr = (s["H"] - dbar*G)/n*k
+    return rms2, JtJ, Jtr, 2*Jtr
+
+
+def _wavefront_result(out, wl, H, W, P, extra):
+    gn = [gauss_newton_wavefront(o, P, x) for o, x in zip(out, wl)]
+    res = dict(rms=np.sqrt(np.maximum([g[0] for g in gn], 0.)).reshape(H, W),
+               JtJ=np.array([g[1] for g in gn]).reshape(H, W, P, P),
+               Jtr=np.array([g[2] for g in gn]).reshape(H, W, P),
+               grad=np.array([g[3] for g in gn]).reshape(H, W, P),
+               n=out[:, 0].reshape(H, W), bad=out[:, -1].reshape(H, W),
+               sums=out.reshape(H, W, -1))
+    res.update(extra)
+    return res
+
+
+def wavefront_jacobian(system, params, heights=(0., .707, 1.), wavelengths=None, nrays=1000,
+                       distribution="hexapolar", clip=False, radius=None, chunk=1 << 20,
+                       engine=None, exact=False):
+    """Exact derivatives of the rms wavefront error of every (height,
+    wavelength) bundle with respect to the parameters `params` [(j, kind)]
+    (tolerance's vocabulary), on the device: the piston-removed rms of opd()'s
+    per-ray wavefront, chief-ray referenced, over the rays whose path and
+    derivatives are finite.
+
+    The sphere is opd()'s default (or of `radius`), centred on the chief
+    ray's image point; its radius and the frame change to the image are held
+    fixed, its centre follows the parameters.  Shape parameters of the image
+    surface and tilts of the last two surfaces are refused (ValueError).  The
+    bundles are generated as spot_jacobian's.  Returns a dict: rms (H, W) in
+    waves, grad (H, W, P) of rms^2, JtJ (H, W, P, P), Jtr (H, W, P), n, bad,
+    sums (H, W, .) the device rows, and heights, wavelengths, params."""
+    eng = engine or default_engine()
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    params = list(params)
+    chunk = int(chunk)
+    if chunk < 1:
+        raise ValueError("chunk must be >= 1")
+    _wavefront_checked(system, wavelengths, params)
+    B = _Bundles(system, heights, wavelengths, nrays, distribution, eng, exact)
+    st = None
+    try:
+        moves = record_tangents(B.nominal, params)
+        st = _Wavefront(eng, system, B, heights, moves, radius, clip, exact)
+        out = _wavefront_sums(eng, B, st, moves, clip, chunk, exact)
+    finally:
+        if st is not None:
+            st.close()
+        B.close()
+    return _wavefront_result(out, st.wl, len(heights), len(wavelengths), len(params),
+                             dict(heights=np.asarray(heights, np.float64),
+                                  wavelengths=np.asarray(wavelengths, np.float64),
+                                  params=params))
+
+
+def _wavefront_merits(eng, B, st, params, deltas, weights, clip, exact):
+    """sum_b w_b rms_b^2 (waves^2) of each row of `deltas` (V, P) on the
+    fixed bundles B: each variant's sphere centred on its chief rays, all
+    marched in one rtx_trace_reduce_many launch; then rtx_trace_opd and
+    rtx_wavefront_sums (P = 0) per variant and bundle, the radius and a0
+    the current lens's"""
+    t = perturbed_tables(B.nominal, params, deltas)
+    V, W, S = t.shape
+    nb = len(B.rays)
+    v, b = np.meshgrid(np.arange(V), np.arange(nb), indexing="ij")
+    v, b = v.reshape(-1), b.reshape(-1)
+    items = np.stack([v*W + b % W, b], -1)
+    m = eng.trace_reduce_many(t.reshape(V*W, S), [(y, u, None) for y, u in st.chief], items,
+                              clip=True, rot0=B.rot0, exact=exact).reshape(V, nb, 20)
+    Nmax = max(y.shape[0] for y, _ in B.rays)
+    A, Pp = eng.empty((Nmax,)), eng.empty((Nmax, 3))
+    rms2 = np.full((V, nb), np.inf)
+    try:
+        for vi in range(V):
+            for bi, (y0, u0) in enumerate(B.rays):
+                w = bi % W
+                if m[vi, bi, 4] != 1:                  # the chief ray is lost
+                    continue
+                spec = dict(st.specs[bi])
+                ti = t[vi, w, -1]
+                t0 = ei = B.nominal[w, -1]
+                x, y = m[vi, bi, 1], m[vi, bi, 2]
+                Y0 = st.yimg[bi]
+                dy = np.array([x - Y0[0], y - Y0[1],
+                               _image_sag(ei, x, y) - _image_sag(ei, Y0[0], Y0[1])])
+                doff = np.asarray(ti["offset"], float) - np.asarray(t0["offset"], float)
+                spec["d"] = np.asarray(spec["d"], float) - doff @ st.Ri.T - dy
+                spec["n_after"] = float(t[vi, w, S - 2]["n"])
+                N = y0.shape[0]
+                eng.trace_opd(t[vi, w, :-1], y0, u0, spec, A, Pp, N=N, clip=clip, rot0=B.rot0,
+                              exact=exact)
+                s = eng.wavefront_sums(A, None, st.a0[bi], N=N)
+                with np.errstate(all="ignore"):
+                    dbar = s["sum_d"]/s["n"]
+                    r2 = (s["sum_d2"]/s["n"] - dbar*dbar)/st.wl[bi]**2
+                rms2[vi, bi] = r2 if s["n"] > 0 else np.inf
+    finally:
+        A.free(), Pp.free()
+    return (weights.reshape(-1)*rms2).sum(1)
+
+
+def optimize_wavefront(system, params, heights=(0., .707, 1.), wavelengths=None, weights=None,
+                       iterations=20, damping=1e-3, nrays=1000, distribution="hexapolar",
+                       clip=False, lambdas=(.1, 1., 10., 100.), chunk=1 << 20, engine=None,
+                       exact=False):
+    """optimize_spot on the merit sum_b w_b rms_b^2 with rms_b the rms
+    wavefront error in waves (wavefront_jacobian's): the same parameters,
+    loop and returns.  Each iteration takes the sphere of the re-aimed lens;
+    the trial steps are scored on the same bundles with that sphere's radius
+    and each variant's own chief-ray centre."""
+    params = _check_kinds(params)
+    eng = engine or default_engine()
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    H, W, P = len(heights), len(wavelengths), len(params)
+    _wavefront_checked(system, wavelengths, params)
+
+    def prepare(system, B, final):
+        moves = None if final else record_tangents(B.nominal, params)
+        st = _Wavefront(eng, system, B, heights, moves, None, clip, exact)
+        st.moves = moves
+        return st
+
+    def jacobian(B, st):
+        out = _wavefront_sums(eng, B, st, st.moves, clip, int(chunk), exact)
+        return _wavefront_result(out, st.wl, H, W, P, {})
+
+    return _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
+               distribution, lambdas, eng, exact, prepare, jacobian,
+               lambda B, st, deltas, w: _wavefront_merits(eng, B, st, params, deltas, w, clip,
+                                                          exact))
