@@ -717,6 +717,65 @@ int rtx_trace_opd_jacobian(rtx_ctx *ctx, const rtx_surface *surf, int S,
 int rtx_wavefront_sums(rtx_ctx *ctx, int64_t N, int P, const void *A, const void *dA,
                        int64_t ld, double a0, double *out);
 
+/* ---- lens-parameter derivatives of the geometric OTF -------------------- */
+/*
+ * The geometric OTF sums of image points q and their derivatives with
+ * respect to P lens parameters, at F arbitrary frequencies:
+ *  q       DEVICE, qstride doubles per ray: 2 for rtx_trace_jacobian's q,
+ *          3 for a keep-LAST row of rtx_trace (its y; only x, y are read)
+ *  J       DEVICE (P, 2, ld), rtx_trace_jacobian's; not read when P = 0
+ *  center  host, 2 doubles, or NULL for 0
+ *  freqs   host, nfreq doubles nu_j (cycles per length unit), any order
+ * With d = fl(q - c), a ray enters iff q and all 2P of its derivatives are
+ * finite.  Over the rays that enter, for axis a in {x, y}:
+ *   S[a, j]     = sum exp(-2 pi i nu_j d_a)
+ *   dS[p, a, j] = sum -2 pi i nu_j J[p, a] exp(-2 pi i nu_j d_a)
+ * dS is the derivative of S with c held fixed.  Moving c multiplies S by a
+ * phase, so |S|, the MTF |S|/n and a polychromatic MTF of wavelengths that
+ * share one centre do not depend on it: d|S|/dp = Re(conj(S) dS/dp)/|S|.
+ * out (host, W = RTX_OTF_JAC_WIDTH(P, F) doubles; complex values as (re, im)):
+ *   out[0]                                 n, the rays that enter
+ *   out[1 + 2 (a F + j) + {0, 1}]          S[a, j]
+ *   out[1 + 4F + 2 ((2p + a) F + j) + {0, 1}]   dS[p, a, j]
+ *   out[W - 1]                             bad: rays with a finite q and a
+ *                                          non-finite derivative (they do
+ *                                          not enter)
+ * zeros for N = 0.  Per ray and (a, j) one sincospi(2 fl(nu_j d_a)); the
+ * kernel sums S and T = sum J e (e = exp(-2 pi i nu d)) and the host forms
+ * dS = -2 pi i nu T from fl(fl(2 pi) nu) T.
+ *
+ * Deterministic: the rays are cut into slots of RTX_OTF_JAC_SLOT; each of
+ * the slot's 8 runs of RTX_OTF_JAC_SLOT/8 rays is summed in ray order, the
+ * runs in order, then the slot sums in slot order (a second kernel; no
+ * atomics).  The bits depend only on q, J, c and the frequencies.  S depends
+ * on P only through which rays enter: with bad = 0 it is the same, bit for
+ * bit, as the P = 0 call's on the same points (either qstride).
+ *
+ * Error bound against the exact sums of the same d, eps = 2^-52,
+ * Phi = max |nu_j d_a| over the rays that enter:
+ *   S:   |S - S_exact|   <= (D + 4 Phi + 3) eps n          per component
+ *   dS:  |dS - dS_exact| <= (D + 4 Phi + 5) eps sum_k 2 pi |nu_j J_k[p, a]|
+ *   D = RTX_OTF_JAC_SLOT/8 + 8 + ceil(N / RTX_OTF_JAC_SLOT)   (summation depth)
+ * D bounds the additions (each component of each partial sum is at most
+ * the sum of the terms' magnitudes); 4 Phi the rounding of nu d, which moves
+ * the phase by at most pi Phi eps; 3 the 2 ulp of each sincospi component
+ * and one more; for dS 2 more for the FMA's product and the host's scaling
+ * by fl(fl(2 pi) nu).  Counts are exact.
+ *
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx or out; NULL
+ * q with N > 0, or NULL J with N > 0 and P > 0; N < 0; P outside
+ * 0..RTX_MAX_PARAMS; qstride not 2 or 3; ld < N with P > 0; nfreq outside
+ * 1..RTX_OTF_MAX_FREQS; a NULL freqs; a non-finite frequency or centre.
+ * The slot sums and a ray mask are kept in the context: RTX_E_NOMEM before
+ * allocating when they do not fit.  Synchronous; rtx_last_kernel_ms covers
+ * the three kernels.
+ */
+#define RTX_OTF_JAC_SLOT 4096 /* rays per slot of the deterministic sum */
+#define RTX_OTF_JAC_WIDTH(P, F) (2 + 4 * (F) + 4 * (P) * (F))
+int rtx_otf_jacobian_sums(rtx_ctx *ctx, int64_t N, int P, const void *q, int qstride,
+                          const void *J, int64_t ld, const double *center, int nfreq,
+                          const double *freqs, double *out);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

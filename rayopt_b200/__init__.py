@@ -19,6 +19,6 @@ from .mtf import geometric_mtf  # noqa: F401
 from .tolerance import (tolerance, perturbed_tables, sensitivity_deltas,  # noqa: F401
                         monte_carlo_deltas, record_tangents)
 from .optimize import (spot_jacobian, optimize_spot, wavefront_jacobian,  # noqa: F401
-                       optimize_wavefront)
+                       optimize_wavefront, mtf_jacobian, optimize_mtf)
 
 __version__ = "0.2.0"

@@ -72,6 +72,7 @@ SYMBOLS = {
     "rtx_trace_opd_jacobian": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _i, _vp, _vp,
                                     _vp, _vp, _vp, _vp, _i64, _u]),
     "rtx_wavefront_sums": (_i, [_vp, _i64, _i, _vp, _vp, _i64, C.c_double, _vp]),
+    "rtx_otf_jacobian_sums": (_i, [_vp, _i64, _i, _vp, _i, _vp, _i64, _vp, _i, _vp, _vp]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),

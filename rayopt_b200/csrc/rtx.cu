@@ -91,6 +91,7 @@ enum {
     WS_OTF,      // rtx_otf_rows: slot sums, then the call's sums and counts
     WS_JAC,      // rtx_trace_jacobian: tangent records, their index, block first rows
     WS_JSUM,     // rtx_jacobian_sums: slot sums, then the call's sums
+    WS_OTFJ,     // rtx_otf_jacobian_sums: slot sums, the call's sums, the ray mask
     WS_COUNT
 };
 
@@ -2233,6 +2234,76 @@ int rtx_wavefront_sums(rtx_ctx* ctx, int64_t N, int P, const void* A, const void
     if (!ctx || !out || N < 0 || (N > 0 && (!A || (P > 0 && !dA)))) return RTX_E_BADARG;
     if (P < 0 || P > RTX_MAX_PARAMS || ld < N) return RTX_E_BADARG;
     return gauss_newton_sums<1>(ctx, N, P, A, dA, ld, a0, 0.0, 4 + 2 * P + P * (P + 1) / 2, out);
+}
+
+int rtx_otf_jacobian_sums(rtx_ctx* ctx, int64_t N, int P, const void* q, int qstride,
+                          const void* J, int64_t ld, const double* center, int nfreq,
+                          const double* freqs, double* out) {
+    if (!ctx || !out || N < 0 || (N > 0 && (!q || (P > 0 && !J)))) return RTX_E_BADARG;
+    if (P < 0 || P > RTX_MAX_PARAMS || (qstride != 2 && qstride != 3) || (P > 0 && ld < N))
+        return RTX_E_BADARG;
+    if (nfreq < 1 || nfreq > RTX_OTF_MAX_FREQS || !freqs) return RTX_E_BADARG;
+    bool finite = !center || (std::isfinite(center[0]) && std::isfinite(center[1]));
+    for (int j = 0; j < nfreq; ++j) finite = finite && std::isfinite(freqs[j]);
+    if (!finite) return RTX_E_BADARG;
+    const int F = nfreq, W = RTX_OTF_JAC_WIDTH(P, F);
+    const long long slots = (N + RTX_OTF_JAC_SLOT - 1) / RTX_OTF_JAC_SLOT;
+    if (slots == 0) {
+        memset(out, 0, (size_t)W * sizeof(double));
+        return 0;
+    }
+    OtfJacDev d;
+    memset(&d, 0, sizeof(d));
+    d.P = P;
+    d.F = F;
+    d.qstride = qstride;
+    d.groups = (2 * F + 31) / 32;
+    d.blocks = P > 0 ? (P + OTF_JAC_PB - 1) / OTF_JAC_PB : 1;
+    d.ld = P > 0 ? ld : 0;
+    d.c[0] = center ? center[0] : 0.0;
+    d.c[1] = center ? center[1] : 0.0;
+    for (int j = 0; j < F; ++j) d.nu[j] = freqs[j];
+    CK(cudaSetDevice(ctx->device));
+    Workspace& ws = ctx->ws[WS_OTFJ];
+    // slot rows | the call's row | the mask (one bit per ray of every slot)
+    const size_t per = (size_t)W * sizeof(double);
+    const size_t mask_bytes = (size_t)slots * (RTX_OTF_JAC_SLOT / 8);
+    if ((unsigned long long)slots >= (SIZE_MAX - mask_bytes) / per - 1) return RTX_E_NOMEM;
+    int rc = reserve(ws, (size_t)(slots + 1) * per + mask_bytes);
+    if (rc) return rc;
+    d.part = (double*)ws.p;
+    double* sums = d.part + slots * W;
+    unsigned* mask = (unsigned*)(sums + W);
+    d.mask = mask;
+    const long long items = slots * d.groups * d.blocks;
+    rc = timed(ctx, [&] {
+        otf_jac_mask_kernel<<<(unsigned)slots, 256, 0, ctx->stream>>>(
+            d, (const double*)q, (const double*)J, N, W, mask);
+        ctx->launches++;
+        int rc = (int)cudaGetLastError();
+        if (rc) return rc;
+        otf_jac_kernel<<<cap_grid(ctx, items, 2), 256, 0, ctx->stream>>>(
+            d, (const double*)q, (const double*)J, N, W, items);
+        ctx->launches++;
+        rc = (int)cudaGetLastError();
+        if (rc) return rc;
+        otf_sum_kernel<<<(W + 255) / 256, 256, 0, ctx->stream>>>(d.part, W, slots, sums);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(out, sums, per, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    // dS = -2 pi i nu T: (re, im) = (2 pi nu T_im, -2 pi nu T_re)
+    for (int p = 0; p < P; ++p)
+        for (int j = 0; j < 2 * F; ++j) {
+            const double k = (2.0 * M_PI) * freqs[j % F];
+            double* t = out + 1 + 4 * F + 2 * (p * 2 * F + j);
+            const double re = t[0], im = t[1];
+            t[0] = k * im;
+            t[1] = -(k * re);
+        }
+    return 0;
 }
 
 }  // extern "C"

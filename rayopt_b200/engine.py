@@ -118,6 +118,17 @@ def wavefront_sums_unpack(out, P):
                 H=out[3 + P:3 + 2*P].copy(), K=K, bad=out[-1], out=out)
 
 
+def otf_jacobian_sums_unpack(out, P, F):
+    """rtx_otf_jacobian_sums' row (include/rtx.h) as a dict: n, bad, S
+    complex (2, F), dS complex (P, 2, F) and the row `out`; rows of several
+    calls may be added first"""
+    out = np.asarray(out, np.float64)
+    S = out[1:1 + 4*F].reshape(2, F, 2)
+    dS = out[1 + 4*F:1 + 4*F + 4*P*F].reshape(P, 2, F, 2)
+    return dict(n=out[0], bad=out[-1], S=S[..., 0] + 1j*S[..., 1], dS=dS[..., 0] + 1j*dS[..., 1],
+                out=out)
+
+
 def spot_shape(spec):
     """(K, nx, ny) of a 2-D record, (K, nx) of a radial one"""
     s = spec[0]
@@ -867,6 +878,35 @@ class Engine:
         check(self.lib.rtx_wavefront_sums(self.ctx, N, P, A.ptr, None if dA is None else dA.ptr,
                                           ld, float(a0), ptr(out)))
         return wavefront_sums_unpack(out, P)
+
+    def otf_jacobian_sums(self, q, J, freqs, center=None, N=None):
+        """rtx_otf_jacobian_sums: the geometric OTF sums of DEVICE image points
+        q at the frequencies `freqs` (F,) about `center` (2,) and their
+        derivatives from J (trace_jacobian's (P, 2, ld); None: P = 0).  q is
+        (N, 2) (trace_jacobian's) or (N, 3) (a keep-LAST row of
+        trace_device; its x, y are read).  Returns a
+        dict of n, bad (rays with a finite q and a non-finite derivative), S
+        complex (2, F), dS complex (P, 2, F) and the raw output row `out`."""
+        N = q.shape[0] if N is None else int(N)
+        qs = q.shape[-1] if len(q.shape) >= 2 else 0
+        if np.dtype(q.dtype) != np.float64 or qs not in (2, 3):
+            raise ValueError("q must be float64 (N, 2) or (N, 3), got %s %s"
+                             % (np.dtype(q.dtype), q.shape))
+        _check_operands(q.dtype, N, q=(q, qs))
+        P, ld = (0, max(N, 1)) if J is None else (J.shape[0], J.shape[-1])
+        if J is not None and (np.dtype(J.dtype) != np.float64 or len(J.shape) != 3
+                              or J.shape[1] != 2 or N > ld):
+            raise ValueError("J must be float64 (P, 2, ld) with ld >= N")
+        freqs = np.ascontiguousarray(np.atleast_1d(freqs), np.float64)
+        F = len(freqs)
+        if freqs.ndim != 1 or not 1 <= F <= OTF_MAX_FREQS or not np.isfinite(freqs).all():
+            raise ValueError("need 1..%d finite frequencies, got %r" % (OTF_MAX_FREQS, freqs))
+        c = None if center is None else np.ascontiguousarray(center, np.float64).reshape(2)
+        out = np.zeros(2 + 4*F + 4*P*F)
+        check(self.lib.rtx_otf_jacobian_sums(self.ctx, N, P, q.ptr, qs,
+                                             None if J is None else J.ptr, ld, ptr(c), F,
+                                             ptr(freqs), ptr(out)))
+        return otf_jacobian_sums_unpack(out, P, F)
 
     def ipc_export(self, darray):
         h = (C.c_ubyte*64)()

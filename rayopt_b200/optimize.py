@@ -34,13 +34,23 @@ one-component sums of rtx_wavefront_sums,
 The sphere's radius and the frame change to the image surface are held at
 their values for the current lens; its centre, the chief ray's image point,
 moves with the parameters.
+
+``mtf_jacobian`` and ``optimize_mtf`` do the same for the geometric MTF at
+chosen frequencies: with d_k = q_k - c along one axis, S(nu) = sum_k
+exp(-2 pi i nu d_k) and dS/dp = sum_k -2 pi i nu dq_k/dp exp(-2 pi i nu d_k)
+(rtx_otf_jacobian_sums, c held fixed).  Moving the centre c multiplies S by a
+phase, so MTF = |S|/n and d MTF/dp = Re(conj(S) dS/dp)/(|S| n) need no
+derivative of c, and neither does the polychromatic MTF of wavelengths that
+share one centre.
 """
 import copy
 
 import numpy as np
 
-from .engine import Engine, default_engine, jacobian_sums_unpack, wavefront_sums_unpack
+from .engine import (OTF_MAX_FREQS, Engine, default_engine, jacobian_sums_unpack,
+                     otf_jacobian_sums_unpack, wavefront_sums_unpack)
 from .lazy import opd_spec
+from .mtf import poly_otf
 from .surface_table import RTX_MAX_ASPH, SURFACE_DTYPE, pack_system
 from .tolerance import _chief, launch_bundles, perturbed_tables, record_tangents
 
@@ -213,18 +223,29 @@ def _check_kinds(params):
     return params
 
 
-def _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
-        distribution, lambdas, eng, exact, prepare, jacobian, merits):
-    """The Levenberg-Marquardt loop of optimize_spot and optimize_wavefront
-    on a copy of `system`.  Per iteration, on the re-aimed bundles B:
-    state = prepare(system, B, final) (freed by state.close() when it has
-    one; `final`: only the merit of the last, re-aimed lens is wanted),
-    jacobian(B, state) the per-bundle normal equations (JtJ (H, W, P, P),
-    Jtr (H, W, P)), merits(B, state, deltas) the weighted merit of each
-    row of deltas on the fixed bundles."""
-    H, W, P = len(heights), len(wavelengths), len(params)
-    weights = np.ones((H, W)) if weights is None else np.broadcast_to(
+def _bundle_weights(weights, H, W):
+    """the per-bundle weights (H, W) of optimize_spot and optimize_wavefront"""
+    return np.ones((H, W)) if weights is None else np.broadcast_to(
         np.asarray(weights, np.float64), (H, W))
+
+
+def _weighted_normal(res, weights):
+    """sum_b w_b of the per-bundle normal equations res["JtJ"] (H, W, P, P)
+    and res["Jtr"] (H, W, P)"""
+    w = weights[..., None, None]
+    return (w*res["JtJ"]).sum((0, 1)), (w[..., 0]*res["Jtr"]).sum((0, 1))
+
+
+def _lm(system, params, heights, wavelengths, iterations, damping, nrays, distribution,
+        lambdas, eng, exact, prepare, normal, merits):
+    """The Levenberg-Marquardt loop of optimize_spot, optimize_wavefront and
+    optimize_mtf on a copy of `system`.  Per iteration, on the re-aimed
+    bundles B: state = prepare(system, B, final) (freed by state.close()
+    when it has one; `final`: only the merit of the last, re-aimed lens is
+    wanted), normal(B, state) the weighted normal equations (JtJ (P, P),
+    Jtr (P,)), merits(B, state, deltas) the weighted merit of each row of
+    deltas on the fixed bundles."""
+    P = len(params)
     system = copy.deepcopy(system)
     total = np.zeros(P)
     hist = dict(merit=[], lam=[], step=[], trial=[])
@@ -235,15 +256,12 @@ def _lm(system, params, heights, wavelengths, weights, iterations, damping, nray
         try:
             state = prepare(system, B, it == iterations)
             if it == iterations:               # the final lens, re-aimed
-                hist["merit"].append(float(merits(B, state, np.zeros((1, P)), weights)[0]))
+                hist["merit"].append(float(merits(B, state, np.zeros((1, P)))[0]))
                 break
-            res = jacobian(B, state)
-            w = weights[..., None, None]
-            JtJ = (w*res["JtJ"]).sum((0, 1))
-            Jtr = (w[..., 0]*res["Jtr"]).sum((0, 1))
+            JtJ, Jtr = normal(B, state)
             lams = [lam*f for f in lambdas]
             steps = np.array([lm_step(JtJ, Jtr, x) for x in lams])
-            merit = merits(B, state, np.vstack([np.zeros(P), steps]), weights)
+            merit = merits(B, state, np.vstack([np.zeros(P), steps]))
         finally:
             if state is not None and hasattr(state, "close"):
                 state.close()
@@ -291,15 +309,17 @@ def optimize_spot(system, params, heights=(0., .707, 1.), wavelengths=None, weig
     wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
     heights = list(heights)
     H, W, P = len(heights), len(wavelengths), len(params)
+    weights = _bundle_weights(weights, H, W)
     record_tangents(_nominal(system, wavelengths)[0], params)  # refusals before any device work
 
-    def jacobian(B, state):
+    def normal(B, state):
         moves = record_tangents(B.nominal, params)
-        return _result(_sums(eng, B, moves, clip, int(chunk), exact), H, W, P, {})
+        return _weighted_normal(_result(_sums(eng, B, moves, clip, int(chunk), exact), H, W, P, {}),
+                                weights)
 
-    return _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
-               distribution, lambdas, eng, exact, lambda system, B, final: None, jacobian,
-               lambda B, state, deltas, w: _merits(eng, B, params, deltas, w, clip, exact))
+    return _lm(system, params, heights, wavelengths, iterations, damping, nrays, distribution,
+               lambdas, eng, exact, lambda system, B, final: None, normal,
+               lambda B, state, deltas: _merits(eng, B, params, deltas, weights, clip, exact))
 
 
 # ---- the rms wavefront error ---------------------------------------------
@@ -577,6 +597,7 @@ def optimize_wavefront(system, params, heights=(0., .707, 1.), wavelengths=None,
     wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
     heights = list(heights)
     H, W, P = len(heights), len(wavelengths), len(params)
+    weights = _bundle_weights(weights, H, W)
     _wavefront_checked(system, wavelengths, params)
 
     def prepare(system, B, final):
@@ -585,11 +606,225 @@ def optimize_wavefront(system, params, heights=(0., .707, 1.), wavelengths=None,
         st.moves = moves
         return st
 
-    def jacobian(B, st):
+    def normal(B, st):
         out = _wavefront_sums(eng, B, st, st.moves, clip, int(chunk), exact)
-        return _wavefront_result(out, st.wl, H, W, P, {})
+        return _weighted_normal(_wavefront_result(out, st.wl, H, W, P, {}), weights)
 
-    return _lm(system, params, heights, wavelengths, weights, iterations, damping, nrays,
-               distribution, lambdas, eng, exact, prepare, jacobian,
-               lambda B, st, deltas, w: _wavefront_merits(eng, B, st, params, deltas, w, clip,
-                                                          exact))
+    return _lm(system, params, heights, wavelengths, iterations, damping, nrays, distribution,
+               lambdas, eng, exact, prepare, normal,
+               lambda B, st, deltas: _wavefront_merits(eng, B, st, params, deltas, weights, clip,
+                                                       exact))
+
+
+# ---- the geometric MTF at chosen frequencies -------------------------------
+def _check_freqs(freqs):
+    nu = np.ascontiguousarray(np.atleast_1d(np.asarray(freqs, np.float64)))
+    if nu.ndim != 1 or not 1 <= len(nu) <= OTF_MAX_FREQS or not np.isfinite(nu).all():
+        raise ValueError("need 1..%d finite frequencies, got %r" % (OTF_MAX_FREQS, freqs))
+    return nu
+
+
+def _spectral(spectral_weights, W):
+    if spectral_weights is None:
+        return np.ones(W)
+    sw = np.asarray(spectral_weights, np.float64)
+    if sw.size != W or not np.isfinite(sw).all():
+        raise ValueError("spectral_weights must be %d finite values, got %r" % (W, spectral_weights))
+    return sw.reshape(W)
+
+
+def _per_residual(name, x, shape):
+    """`x` broadcast to (H, 2, F), ValueError when it does not"""
+    try:
+        return np.broadcast_to(np.asarray(x, np.float64), shape)
+    except ValueError:
+        raise ValueError("%s of shape %s does not broadcast to (heights, 2, freqs) = %s"
+                         % (name, np.shape(x), shape)) from None
+
+
+def _otf_sums(eng, B, moves, freqs, clip, chunk, exact):
+    """(bundles, W) rtx_otf_jacobian_sums rows of every bundle about its
+    height's chief ray at wavelengths[0], its ray chunks added on the host in
+    chunk order"""
+    P, F = len(moves), len(freqs)
+    out = np.zeros((len(B.rays), 2 + 4*F + 4*P*F))
+    for b, (y0, u0) in enumerate(B.rays):
+        w = b % B.W
+        mv = [[(row, rec[w]) for row, rec in m] for m in moves]
+        N = y0.shape[0]
+        for r0 in range(0, N, chunk):
+            r1 = min(N, r0 + chunk)
+            q, J = eng.trace_jacobian(B.nominal[w], y0.rows(r0, r1), u0.rows(r0, r1), mv,
+                                      clip=clip, rot0=B.rot0, exact=exact)
+            try:
+                out[b] += eng.otf_jacobian_sums(q, J, freqs, B.centers[b - w, :2])["out"]
+            finally:
+                q.free(), J.free()
+    return out
+
+
+def _abs_grad(S, dS):
+    """|S| and d|S| = Re(conj(S) dS)/|S|: S (..., 2, F), dS (..., P, 2, F)
+    complex; the gradient (..., 2, F, P), NaN where |S| = 0"""
+    a = np.abs(S)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        g = (np.conj(S)[..., None, :, :]*dS).real/a[..., None, :, :]
+        g = np.where(a[..., None, :, :] > 0, g, np.nan)
+    return a, np.moveaxis(g, -3, -1)
+
+
+def _mtf_result(out, H, W, P, F, sw):
+    u = [otf_jacobian_sums_unpack(o, P, F) for o in out]
+    n = np.array([x["n"] for x in u]).reshape(H, W)
+    S = np.array([x["S"] for x in u]).reshape(H, W, 2, F)
+    dS = np.array([x["dS"] for x in u]).reshape(H, W, P, 2, F)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        otf = S/n[..., None, None]
+        dotf = dS/n[..., None, None, None]
+    _, grad = _abs_grad(otf, dotf)
+    poly = poly_otf(otf[:, :, None], n[:, :, None], sw)[:, 0]
+    wk = np.where(n > 0, sw, 0.)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        dpoly = np.einsum("hw,hwpaf->hpaf", wk, np.where(wk[..., None, None, None] > 0, dotf, 0)) \
+            / wk.sum(1)[:, None, None, None]
+    poly_mtf, poly_grad = _abs_grad(poly, dpoly)
+    return dict(otf=otf, mtf=np.abs(otf), grad=grad, poly=poly, poly_mtf=poly_mtf,
+                poly_grad=poly_grad, n=n, bad=out[:, -1].reshape(H, W), sums=out.reshape(H, W, -1))
+
+
+def mtf_jacobian(system, params, freqs, heights=(0., .707, 1.), wavelengths=None, nrays=1000,
+                 distribution="hexapolar", clip=True, spectral_weights=None, chunk=1 << 20,
+                 engine=None, exact=False):
+    """Exact derivatives of the geometric MTF of every (height, wavelength)
+    bundle at the frequencies `freqs` (cycles per length unit) with respect
+    to the parameters `params` [(j, kind)] (tolerance's vocabulary), on the
+    device.
+
+    The bundles are spot_jacobian's; each is marched with tangents in chunks
+    of `chunk` rays (rtx_trace_jacobian) and reduced to the OTF sums S and
+    their derivatives dS (rtx_otf_jacobian_sums), the chunks added on the
+    host in order.  As in geometric_mtf, every wavelength of a height is
+    centred on that height's chief ray at wavelengths[0].  The MTF |S|/n does
+    not depend on the centre, so its derivative Re(conj(S) dS)/(|S| n) needs
+    none of the centre's.  With clip=True (the default) the MTF is
+    geometric_mtf's at defocus 0.
+
+    Returns a dict: freq (F,), otf complex (H, W, 2, F) (axis 0: x, 1: y),
+    mtf = |otf|, grad (H, W, 2, F, P) of the MTF, poly (H, 2, F) the
+    `spectral_weights` mean of the wavelengths' OTFs (mtf.poly_otf),
+    poly_mtf = |poly|, poly_grad (H, 2, F, P), n (H, W) the rays that enter,
+    bad (H, W) the rays with a finite image point and a non-finite
+    derivative, sums (H, W, .) the device rows, and heights, wavelengths,
+    params.  Where |S| = 0 the MTF has no derivative: grad (and poly_grad
+    where |poly| = 0) is NaN there."""
+    eng = engine or default_engine()
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    params = list(params)
+    nu = _check_freqs(freqs)
+    sw = _spectral(spectral_weights, len(wavelengths))
+    chunk = int(chunk)
+    if chunk < 1:
+        raise ValueError("chunk must be >= 1")
+    moves = record_tangents(_nominal(system, wavelengths)[0], params)  # refusals first
+    B = _Bundles(system, heights, wavelengths, nrays, distribution, eng, exact)
+    try:
+        out = _otf_sums(eng, B, moves, nu, clip, chunk, exact)
+    finally:
+        B.close()
+    res = _mtf_result(out, len(heights), len(wavelengths), len(params), len(nu), sw)
+    res.update(freq=nu, heights=np.asarray(heights, np.float64),
+               wavelengths=np.asarray(wavelengths, np.float64), params=params)
+    return res
+
+
+def mtf_normal(mtf, grad, targets, weights):
+    """The Gauss-Newton normal equations of sum w (t - M)^2 over the
+    residuals (any shape; `targets` and `weights` broadcast to it):
+    JtJ = sum w g g^T, Jtr = -sum w g (t - M) with g = grad (..., P) =
+    dM/dp.  Residuals with a non-finite M or gradient are left out."""
+    M = np.asarray(mtf, np.float64)
+    g = np.asarray(grad, np.float64)
+    ok = np.isfinite(g).all(-1) & np.isfinite(M)
+    g, w = g[ok], np.broadcast_to(np.asarray(weights, np.float64), M.shape)[ok]
+    r = (np.broadcast_to(np.asarray(targets, np.float64), M.shape) - M)[ok]
+    return np.einsum("k,ka,kb->ab", w, g, g), -np.einsum("k,ka,k->a", w, g, r)
+
+
+def _trial_mtf(eng, B, params, deltas, freqs, sw, clip, exact):
+    """the polychromatic MTF (V, H, 2, F) of each row of `deltas` (V, P) on
+    the fixed bundles B: every variant marched keep-LAST (rtx_trace_batch,
+    up to 8 bundles per launch), then rtx_otf_jacobian_sums with P = 0 about
+    the current lens's centres"""
+    t = perturbed_tables(B.nominal, params, deltas)
+    V, W = t.shape[:2]
+    nb, F = len(B.rays), len(freqs)
+    Ns = [y.shape[0] for y, _ in B.rays]
+    ld = max(64, -(-max(Ns)//64)*64)
+    Ys = [eng.empty((1, ld, 3)) for _ in range(min(nb, 8))]
+    out = np.zeros((V, nb, 2 + 4*F))
+    try:
+        for v in range(V):
+            for b0 in range(0, nb, 8):
+                bs = range(b0, min(nb, b0 + 8))
+                eng.trace_device_batch([t[v, b % W] for b in bs], [B.rays[b][0] for b in bs],
+                                       [B.rays[b][1] for b in bs], Ys[:len(bs)], None, None, None,
+                                       Ns=[Ns[b] for b in bs], ld=ld, clip=clip, keep_last=True,
+                                       rot0=B.rot0, exact=exact)
+                for i, b in enumerate(bs):
+                    out[v, b] = eng.otf_jacobian_sums(Ys[i].rows(0), None, freqs,
+                                                      B.centers[b - b % W, :2], N=Ns[b])["out"]
+    finally:
+        for y in Ys:
+            y.free()
+    return np.array([_mtf_result(o, nb//W, W, 0, F, sw)["poly_mtf"] for o in out])
+
+
+def _mtf_merits(eng, B, params, deltas, freqs, sw, targets, weights, clip, exact):
+    """sum w (t - polyMTF)^2 of each row of `deltas` (V, P) on the fixed
+    bundles B (_trial_mtf); a residual without rays counts as inf"""
+    M = _trial_mtf(eng, B, params, deltas, freqs, sw, clip, exact)
+    r2 = np.where(np.isfinite(M), (targets - M)**2, np.inf)
+    return np.where(weights > 0, weights*r2, 0.).sum((1, 2, 3))
+
+
+def optimize_mtf(system, params, freqs, targets=1., heights=(0., .707, 1.), wavelengths=None,
+                 weights=None, iterations=20, damping=1e-3, nrays=1000, distribution="hexapolar",
+                 clip=True, spectral_weights=None, lambdas=(.1, 1., 10., 100.), chunk=1 << 20,
+                 engine=None, exact=False):
+    """Levenberg-Marquardt on sum_h sum_a sum_j w (t_j - polyMTF_h,a(nu_j))^2,
+    the polychromatic MTF of mtf_jacobian at the frequencies `freqs`, both
+    axes (x, y) and every height.
+
+    `targets` and `weights` (default 1) broadcast to (H, 2, F).  The
+    parameters, loop and returns are optimize_spot's: each iteration re-aims
+    the lens, takes mtf_jacobian's poly_grad g and solves with
+    JtJ = sum w g g^T and Jtr = -sum w g (t - M) (mtf_normal; residuals with
+    a NaN gradient are left out), scores the trial steps on the same bundles
+    with the current lens's centres and applies the best one if it lowers
+    the merit.  A residual at a height that no ray reaches counts as inf.
+    The caller's System is not modified."""
+    params = _check_kinds(params)
+    eng = engine or default_engine()
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    H, W, P = len(heights), len(wavelengths), len(params)
+    nu = _check_freqs(freqs)
+    F = len(nu)
+    targets = _per_residual("targets", targets, (H, 2, F))
+    weights = _per_residual("weights", 1. if weights is None else weights, (H, 2, F))
+    sw = _spectral(spectral_weights, W)
+    chunk = int(chunk)
+    if chunk < 1:
+        raise ValueError("chunk must be >= 1")
+    record_tangents(_nominal(system, wavelengths)[0], params)  # refusals before any device work
+
+    def normal(B, state):
+        out = _otf_sums(eng, B, record_tangents(B.nominal, params), nu, clip, chunk, exact)
+        res = _mtf_result(out, H, W, P, F, sw)
+        return mtf_normal(res["poly_mtf"], res["poly_grad"], targets, weights)
+
+    return _lm(system, params, heights, wavelengths, iterations, damping, nrays, distribution,
+               lambdas, eng, exact, lambda system, B, final: None, normal,
+               lambda B, state, deltas: _mtf_merits(eng, B, params, deltas, nu, sw, targets,
+                                                    weights, clip, exact))
