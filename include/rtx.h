@@ -1002,6 +1002,107 @@ int rtx_opd_points(rtx_ctx *ctx, int dtype, int64_t N, const void *A, const void
 int rtx_grid_range(rtx_ctx *ctx, int dtype, int64_t n, const void *o, int64_t *count,
                    double *lo, double *hi);
 
+/* ---- diffraction PSF by direct summation over the exit-pupil rays -------- */
+/*
+ * The Debye (Fourier) sum of the pupil function over the traced rays
+ * themselves, on an image grid the caller chooses, through focus.  Inputs are
+ * rtx_trace_opd's A (N,) and P (N,3) (DEVICE, FP64): P in the image frame
+ * relative to the sphere centre, the chief ray's image point, so that
+ * s_j = -P_j/R is the unit direction from the ray's sphere point to the
+ * centre.  With the optional DEVICE weights w (N,) (NULL: all 1),
+ *   U_k(a, b) = sum_j w_j exp(2 pi i [ (A_j - a0)/lambda
+ *                                     + kappa (sx_j p_a + sy_j q_b + sz_j z_k) ])
+ *   p_a = p0 + a dp (a < nx),  q_b = q0 + b dq (b < ny),  k < planes
+ * over the rays whose A_j, P_j and w_j are finite; the others are left out
+ * and counted.  a0 is the chief ray's A (it keeps the phases small), lambda
+ * the wavelength in lens units, kappa = n_image/lambda, R the sphere radius
+ * (rtx_opd.radius).  This is the first order in the image point X of
+ * n |X - P_j|; +z is along the image frame's z, as in rtx_spot_rows.
+ * At z = 0 on the grid p_a = fftfreq(nx, dx kappa/R) of a regridded OPD o
+ * (nodes x_m = x_0 + m dx used as rays, w = 1, A = a0 - lambda o), rtx_psf's
+ * PSF is |U|^2/(n nx ny) exactly (n the finite nodes): the FFT's own phase
+ * convention, up to a unit phase per pixel.  The intensity in Strehl units is
+ * I = |U|^2/(sum w)^2: 1 at the chief point for an aberration-free pupil.
+ */
+#define RTX_PUPIL_MAX_PLANES 16
+#define RTX_PUPIL_MAX_PIXELS 4096  /* nx, ny */
+#define RTX_PUPIL_CHUNK      32    /* rays summed into a fresh accumulator */
+#define RTX_PUPIL_SLOT       2048  /* least rays per slot */
+#define RTX_PUPIL_MAX_SLOTS  16
+typedef struct rtx_pupil {
+    int32_t planes;                  /* K in 1..16 */
+    int32_t reserved;                /* 0 */
+    int64_t nx, ny;                  /* 1..RTX_PUPIL_MAX_PIXELS */
+    double a0;                       /* reference path (the chief ray's A) */
+    double wavelength;               /* lambda in lens units */
+    double kappa;                    /* n_image/lambda */
+    double radius;                   /* R */
+    double p0, dp, q0, dq;           /* p_a = p0 + a dp, q_b = q0 + b dq */
+    double z[RTX_PUPIL_MAX_PLANES];  /* defocus distances */
+} rtx_pupil;
+size_t rtx_sizeof_pupil(void);
+
+/*
+ * rtx_pupil_sum ADDS U to the DEVICE complex (K, nx, ny) array U (re, im
+ * interleaved, 2 K nx ny doubles) and writes *count (rays summed) and *sumw
+ * (their sum of w; the count when w is NULL) on the host.  Calls add up, so
+ * a bundle can be summed in chunks of rays (memory is bounded by the chunk).
+ * Synchronous; rtx_last_kernel_ms covers both kernels.
+ *
+ * Kernel: per plane U_k = X^T diag(c_k) Y, X_j(a) = exp(2 pi i kappa sx_j
+ * p_a), Y_j(b) = exp(2 pi i kappa sy_j q_b), c_kj = w_j exp(2 pi i [(A_j -
+ * a0)/lambda + kappa sz_j z_k]): an (nx x N)(N x ny) complex product on the
+ * FP64 tensor cores (mma m16n8k16).  X and Y of RTX_PUPIL_CHUNK rays are made
+ * in shared memory once per chunk, with one sincospi per block of 8 pixels
+ * stepped by the phasor of dp (dq), and serve up to 8 planes (K > 8 runs
+ * ceil(K/8) plane groups).
+ *
+ * Deterministic: the rays are cut into slots of L = max(RTX_PUPIL_SLOT,
+ * ceil(N/RTX_PUPIL_MAX_SLOTS)) rays rounded up to RTX_PUPIL_CHUNK; within a
+ * slot each chunk is summed into a fresh accumulator and added to the slot's
+ * sum in chunk order; a second kernel adds the slots in slot order and then
+ * the result to U (no atomics).  The bits depend only on A, P, w, N and the
+ * record, not on the launch grid, the context or the call.
+ *
+ * Error bound, eps = 2^-52, per component of the sum one call adds:
+ *   |U - U_exact| <= (D + 24 Phi + 40) eps sum |w|
+ *   D = 2 RTX_PUPIL_CHUNK + ceil(L/RTX_PUPIL_CHUNK) + slots + 1  (summation depth)
+ *   Phi = max over the summed rays of |A_j - a0|/|lambda| + |kappa| (|sx_j|
+ *         (|p0| + (nx-1)|dp|) + |sy_j| (|q0| + (ny-1)|dq|) + |sz_j| max|z_k|)
+ * 24 Phi bounds the rounding of the phases (4 pi Phi for c, 7 pi Phi for each
+ * of X and Y, whose steps carry the step phase's error through 7 products);
+ * 40 the sincospi, product and step roundings of one term.
+ *
+ * RTX_E_BADARG, before any device work or allocation: NULL ctx, spec, U,
+ * count or sumw; N < 0; NULL A or P with N > 0; planes outside 1..16; nx or
+ * ny outside 1..RTX_PUPIL_MAX_PIXELS; reserved != 0; a zero or non-finite
+ * wavelength or radius; a non-finite a0, kappa, p0, dp, q0, dq or z.  N = 0
+ * adds nothing and launches nothing.  The slot sums (slots (2 K nx ny + 2)
+ * doubles) are kept in the context: RTX_E_NOMEM before allocating them when
+ * they do not fit in free device memory.
+ */
+int rtx_pupil_sum(rtx_ctx *ctx, int64_t N, const double *A, const double *P,
+                  const double *w, const rtx_pupil *spec, double *U, int64_t *count,
+                  double *sumw);
+
+/*
+ * I = scale |U_k(a, b)|^2 ADDED to the DEVICE (K, nx, ny) PSF psf, for the
+ * complex U of rtx_pupil_sum on the grid of `spec` (scale = 1/(sum w)^2 gives
+ * Strehl units; calls for several wavelengths with their spectral weights
+ * accumulate a polychromatic PSF).  stats (host, (K, 5) doubles, or NULL)
+ * receives per plane, over the PSF after the addition: sum psf, max psf, the
+ * flat index a ny + b of its first maximum, sum psf p_a and sum psf q_b.  The
+ * sums are taken in a fixed order (fixed blocks of pixels, fixed tree order,
+ * the blocks in order on the host): the same inputs give the same bits.
+ * RTX_E_BADARG before any device work for a NULL ctx, spec, U or psf, a
+ * record rtx_pupil_sum refuses, or a non-finite scale.  Scratch of
+ * K ceil(nx ny/2048) 5 doubles is kept in the context; RTX_E_NOMEM before
+ * allocating it when it does not fit.  Synchronous; rtx_last_kernel_ms gives
+ * the device time of the call.
+ */
+int rtx_pupil_intensity(rtx_ctx *ctx, const rtx_pupil *spec, const double *U, double scale,
+                        double *psf, double *stats);
+
 #ifdef __cplusplus
 }
 #endif

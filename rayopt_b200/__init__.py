@@ -16,6 +16,7 @@ from ._lib import RtxError  # noqa: F401
 from .spot import spots  # noqa: F401
 from .opd import opds  # noqa: F401
 from .mtf import geometric_mtf  # noqa: F401
+from .psf import psfs  # noqa: F401
 from .tolerance import (tolerance, perturbed_tables, sensitivity_deltas,  # noqa: F401
                         monte_carlo_deltas, record_tangents)
 from .optimize import (spot_jacobian, optimize_spot, wavefront_jacobian,  # noqa: F401

@@ -24,6 +24,7 @@ SYMBOLS = {
     "rtx_sizeof_opd": (_sz, []),
     "rtx_sizeof_spot": (_sz, []),
     "rtx_sizeof_otf": (_sz, []),
+    "rtx_sizeof_pupil": (_sz, []),
     "rtx_device_count": (_i, []),
     "rtx_strerror": (C.c_char_p, [_i]),
     "rtx_surface_finalize": (_i, [_vp, _i, _vp]),
@@ -73,6 +74,8 @@ SYMBOLS = {
                                     _vp, _vp, _vp, _vp, _i64, _u]),
     "rtx_wavefront_sums": (_i, [_vp, _i64, _i, _vp, _vp, _i64, C.c_double, _vp]),
     "rtx_otf_jacobian_sums": (_i, [_vp, _i64, _i, _vp, _i, _vp, _i64, _vp, _i, _vp, _vp]),
+    "rtx_pupil_sum": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rtx_pupil_intensity": (_i, [_vp, _vp, _vp, C.c_double, _vp, _vp]),
     "rtx_selftest_math": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "rtx_selftest_math2": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "rtx_aim_plan": (_i, [_vp, _vp, _i64, _vp, C.POINTER(_i64)]),
@@ -125,8 +128,8 @@ def load():
     if lib.rtx_sizeof_aim() != aim_dtype().itemsize:
         raise RtxError("rtx_aim layout mismatch: C %d, numpy %d" % (
             lib.rtx_sizeof_aim(), aim_dtype().itemsize))
-    from .engine import OTF_DTYPE, SPOT_DTYPE
-    for name, dt in (("spot", SPOT_DTYPE), ("otf", OTF_DTYPE)):
+    from .engine import OTF_DTYPE, PUPIL_DTYPE, SPOT_DTYPE
+    for name, dt in (("spot", SPOT_DTYPE), ("otf", OTF_DTYPE), ("pupil", PUPIL_DTYPE)):
         if getattr(lib, "rtx_sizeof_" + name)() != dt.itemsize:
             raise RtxError("rtx_%s layout mismatch: C %d, numpy %d" % (
                 name, getattr(lib, "rtx_sizeof_" + name)(), dt.itemsize))

@@ -6,6 +6,7 @@
 #include "rtx_device.cuh"
 #include "rtx_psf.cuh"
 #include "rtx_delaunay.cuh"
+#include "rtx_pupil.cuh"
 
 #include <cufft.h>  // types only: the library is opened at run time (rtx_psf)
 #include <dlfcn.h>
@@ -92,6 +93,8 @@ enum {
     WS_JAC,      // rtx_trace_jacobian: tangent records, their index, block first rows
     WS_JSUM,     // rtx_jacobian_sums: slot sums, then the call's sums
     WS_OTFJ,     // rtx_otf_jacobian_sums: slot sums, the call's sums, the ray mask
+    WS_PUPIL,    // rtx_pupil_sum: slot sums of U, counts and sum w
+    WS_PUPIL_RED, // rtx_pupil_intensity: per-block sums, maxima and moments
     WS_COUNT
 };
 
@@ -982,6 +985,7 @@ size_t rtx_sizeof_aim(void) { return sizeof(rtx_aim); }
 size_t rtx_sizeof_opd(void) { return sizeof(rtx_opd); }
 size_t rtx_sizeof_spot(void) { return sizeof(rtx_spot); }
 size_t rtx_sizeof_otf(void) { return sizeof(rtx_otf); }
+size_t rtx_sizeof_pupil(void) { return sizeof(rtx_pupil); }
 
 int rtx_device_count(void) {
     int n = 0;
@@ -2906,6 +2910,153 @@ int rtx_grid_range(rtx_ctx* ctx, int dtype, int64_t n, const void* o, int64_t* c
     *count = (int64_t)acc[0];
     *lo = acc[0] ? value(acc[1]) : NAN;
     *hi = acc[0] ? value(acc[2]) : NAN;
+    return 0;
+}
+
+}  // extern "C"
+
+namespace {
+// rtx_pupil_sum's and rtx_pupil_intensity's record check (include/rtx.h)
+bool pupil_ok(const rtx_pupil* s) {
+    if (!s || s->planes < 1 || s->planes > RTX_PUPIL_MAX_PLANES || s->reserved != 0) return false;
+    if (s->nx < 1 || s->nx > RTX_PUPIL_MAX_PIXELS || s->ny < 1 || s->ny > RTX_PUPIL_MAX_PIXELS)
+        return false;
+    if (!std::isfinite(s->wavelength) || s->wavelength == 0.0 || !std::isfinite(s->radius) ||
+        s->radius == 0.0)
+        return false;
+    bool finite = std::isfinite(s->a0) && std::isfinite(s->kappa) && std::isfinite(s->p0) &&
+                  std::isfinite(s->dp) && std::isfinite(s->q0) && std::isfinite(s->dq);
+    for (int k = 0; k < s->planes; ++k) finite = finite && std::isfinite(s->z[k]);
+    return finite;
+}
+
+template <int WR, int WC>
+int launch_pupil_sum(rtx_ctx* ctx, PupilDev& d) {
+    using SM = PupilSmem<WR, WC>;
+    d.tiles_x = (int)((d.nx + SM::TA - 1) / SM::TA);
+    d.tiles_y = (int)((d.ny + SM::TB - 1) / SM::TB);
+    const long long items = d.slots * d.groups * d.tiles_x * d.tiles_y;
+    const size_t smem = (size_t)SM::doubles * sizeof(double);
+    auto kern = pupil_sum_kernel<WR, WC>;
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<(unsigned)items, PUP_THREADS, smem, ctx->stream>>>(d);
+    ctx->launches++;
+    return (int)cudaGetLastError();
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_pupil_sum(rtx_ctx* ctx, int64_t N, const double* A, const double* P, const double* w,
+                  const rtx_pupil* spec, double* U, int64_t* count, double* sumw) {
+    if (!ctx || !spec || !U || !count || !sumw || N < 0 || (N > 0 && (!A || !P)))
+        return RTX_E_BADARG;
+    if (!pupil_ok(spec)) return RTX_E_BADARG;
+    *count = 0;
+    *sumw = 0.0;
+    if (N == 0) return 0;
+    PupilDev d;
+    memset(&d, 0, sizeof(d));
+    d.K = spec->planes;
+    d.groups = (d.K + PUP_GROUP - 1) / PUP_GROUP;
+    d.KG = (d.K + d.groups - 1) / d.groups;
+    d.nx = spec->nx;
+    d.ny = spec->ny;
+    d.N = N;
+    long long L = std::max<long long>(RTX_PUPIL_SLOT, (N + RTX_PUPIL_MAX_SLOTS - 1) / RTX_PUPIL_MAX_SLOTS);
+    d.L = (L + PUP_CH - 1) / PUP_CH * PUP_CH;
+    d.slots = (N + d.L - 1) / d.L;
+    d.a0 = spec->a0;
+    d.lambda = spec->wavelength;
+    d.kappa = spec->kappa;
+    d.radius = spec->radius;
+    d.p0 = spec->p0;
+    d.dp = spec->dp;
+    d.q0 = spec->q0;
+    d.dq = spec->dq;
+    for (int k = 0; k < d.K; ++k) d.z[k] = spec->z[k];
+    d.A = A;
+    d.P = P;
+    d.w = w;
+    CK(cudaSetDevice(ctx->device));
+    const long long n = 2LL * d.K * d.nx * d.ny, row = n + 2;
+    int rc = reserve(ctx->ws[WS_PUPIL], (size_t)(d.slots * row) * sizeof(double));
+    if (rc) return rc;
+    d.part = (double*)ctx->ws[WS_PUPIL].p;
+    rc = timed(ctx, [&] {
+        int rc;
+        if (d.KG == 1)
+            rc = launch_pupil_sum<2, 4>(ctx, d);
+        else if (d.KG == 2)
+            rc = launch_pupil_sum<2, 2>(ctx, d);
+        else if (d.KG <= 4)
+            rc = launch_pupil_sum<1, 2>(ctx, d);
+        else
+            rc = launch_pupil_sum<1, 1>(ctx, d);
+        if (rc) return rc;
+        pupil_fold_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d.part, row, n,
+                                                                             d.slots, U);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
+    std::vector<double> h((size_t)(2 * d.slots));
+    CK(cudaMemcpy2DAsync(h.data(), 2 * sizeof(double), d.part + n, row * sizeof(double),
+                         2 * sizeof(double), (size_t)d.slots, cudaMemcpyDeviceToHost,
+                         ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    double c = 0.0, sw = 0.0;
+    for (long long q = 0; q < d.slots; ++q) {
+        c += h[(size_t)(2 * q)];
+        sw += h[(size_t)(2 * q + 1)];
+    }
+    *count = (int64_t)c;
+    *sumw = sw;
+    return 0;
+}
+
+int rtx_pupil_intensity(rtx_ctx* ctx, const rtx_pupil* spec, const double* U, double scale,
+                        double* psf, double* stats) {
+    if (!ctx || !U || !psf || !pupil_ok(spec) || !std::isfinite(scale)) return RTX_E_BADARG;
+    const int K = spec->planes;
+    const long long npix = spec->nx * spec->ny;
+    const long long nb = (npix + PUP_RED - 1) / PUP_RED;
+    CK(cudaSetDevice(ctx->device));
+    Workspace& ws = ctx->ws[WS_PUPIL_RED];
+    const size_t bytes = (size_t)(K * nb * 5) * sizeof(double);
+    int rc = reserve(ws, bytes);
+    if (rc) return rc;
+    double* part = (double*)ws.p;
+    rc = timed(ctx, [&] {
+        pupil_intensity_kernel<<<dim3((unsigned)nb, (unsigned)K), 256, 0, ctx->stream>>>(
+            U, scale, psf, spec->nx, spec->ny, spec->p0, spec->dp, spec->q0, spec->dq, part);
+        ctx->launches++;
+        return (int)cudaGetLastError();
+    });
+    if (rc) return rc;
+    std::vector<double> h((size_t)(K * nb * 5));
+    CK(cudaMemcpyAsync(h.data(), part, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (stats)
+        for (int k = 0; k < K; ++k) {
+            double sum = 0.0, mx = -1.0, at = -1.0, sp = 0.0, sq = 0.0;
+            for (long long b = 0; b < nb; ++b) {
+                const double* r = &h[(size_t)((k * nb + b) * 5)];
+                sum += r[0];
+                sp += r[3];
+                sq += r[4];
+                if (r[1] > mx) {
+                    mx = r[1];
+                    at = r[2];
+                }
+            }
+            double* o = stats + 5 * k;
+            o[0] = sum;
+            o[1] = mx;
+            o[2] = at;
+            o[3] = sp;
+            o[4] = sq;
+        }
     return 0;
 }
 

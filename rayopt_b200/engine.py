@@ -84,6 +84,50 @@ def otf_spec(z, dnu, nfreq, c, offsets=None):
     return rec
 
 
+# mirrors `struct rtx_pupil` (include/rtx.h)
+PUPIL_MAX_PLANES, PUPIL_MAX_PIXELS = 16, 4096
+PUPIL_CHUNK, PUPIL_SLOT, PUPIL_MAX_SLOTS = 32, 2048, 16
+PUPIL_DTYPE = np.dtype([("planes", "<i4"), ("reserved", "<i4"), ("nx", "<i8"), ("ny", "<i8"),
+                        ("a0", "<f8"), ("wavelength", "<f8"), ("kappa", "<f8"), ("radius", "<f8"),
+                        ("p0", "<f8"), ("dp", "<f8"), ("q0", "<f8"), ("dq", "<f8"),
+                        ("z", "<f8", (PUPIL_MAX_PLANES,))], align=True)
+
+
+def pupil_spec(z, pixels, p0, dp, q0, dq, a0, wavelength, kappa, radius):
+    """An rtx_pupil record: defocus distances `z` (K,), the grid p_a = p0 +
+    a dp, q_b = q0 + b dq of `pixels` (nx, ny), the reference path a0, the
+    wavelength and kappa = n_image/wavelength in lens units and the sphere
+    radius.  Raises ValueError for what rtx_pupil_sum refuses."""
+    z = np.atleast_1d(np.asarray(z, np.float64))
+    nx, ny = (int(v) for v in pixels)
+    if z.ndim != 1 or not 1 <= len(z) <= PUPIL_MAX_PLANES:
+        raise ValueError("need 1..%d planes, got %d" % (PUPIL_MAX_PLANES, len(z)))
+    if not (1 <= nx <= PUPIL_MAX_PIXELS and 1 <= ny <= PUPIL_MAX_PIXELS):
+        raise ValueError("pixels must be in 1..%d, got %r" % (PUPIL_MAX_PIXELS, (nx, ny)))
+    v = np.array([p0, dp, q0, dq, a0, wavelength, kappa, radius], np.float64)
+    if not (np.isfinite(v).all() and np.isfinite(z).all()) or wavelength == 0 or radius == 0:
+        raise ValueError("grid, a0, kappa and z must be finite, wavelength and radius "
+                         "finite and non-zero")
+    rec = np.zeros(1, PUPIL_DTYPE)
+    rec["planes"], rec["nx"], rec["ny"] = len(z), nx, ny
+    for k, x in zip(("p0", "dp", "q0", "dq", "a0", "wavelength", "kappa", "radius"), v):
+        rec[k] = x
+    rec["z"][0, :len(z)] = z
+    return rec
+
+
+def pupil_bound(N, phi, sum_abs_w, chunks=1):
+    """The error bound of include/rtx.h on every component of the U one
+    rtx_pupil_sum call of N rays adds, ``(D + 24 phi + 40) eps sum|w|``,
+    plus ``chunks - 1`` for calls added in order; `phi` the largest phase
+    sum of include/rtx.h over the summed rays"""
+    L = max(PUPIL_SLOT, -(-int(N)//PUPIL_MAX_SLOTS))
+    L = -(-L//PUPIL_CHUNK)*PUPIL_CHUNK
+    slots = -(-int(N)//L)
+    D = 2*PUPIL_CHUNK + -(-L//PUPIL_CHUNK) + slots + 1 + chunks - 1
+    return (D + 24*np.asarray(phi, np.float64) + 40)*2.**-52*np.asarray(sum_abs_w)
+
+
 def otf_bound(spec, N, count, phi, chunks=1):
     """The error bound of include/rtx.h on every component of S, per plane
     (K,): ``(D + 13 phi + 5 RTX_OTF_BLOCK) eps count`` with the summation
@@ -806,6 +850,42 @@ class Engine:
         check(self.lib.rtx_otf_rows(self.ctx, _code(y.dtype), N, y.ptr, inc.ptr, ptr(spec),
                                     ptr(sums), ptr(count)))
         return sums[..., 0] + 1j*sums[..., 1], count
+
+    pupil_spec = staticmethod(pupil_spec)
+
+    def pupil_sum(self, A, P, spec, U, w=None, N=None):
+        """rtx_pupil_sum: ADD the Debye sum U_k(a, b) of the DEVICE rays A
+        (N,), P (N, 3) (rtx_trace_opd's outputs) with optional DEVICE weights
+        w (N,) on the grid and planes of `spec` (pupil_spec) to the complex128
+        DeviceArray U (K, nx, ny).  Returns (count, sum_w) of the rays summed."""
+        N = A.shape[0] if N is None else int(N)
+        _check_operands(np.float64, N, A=(A, 1), P=(P, 3), w=(w, 1))
+        spec = np.ascontiguousarray(spec, PUPIL_DTYPE).reshape(1)
+        s = spec[0]
+        need = int(s["planes"])*int(s["nx"])*int(s["ny"])
+        if np.dtype(U.dtype) != np.complex128 or U.nbytes//16 < need:
+            raise ValueError("U must be a complex128 device array of %d values" % need)
+        count, sumw = C.c_int64(), C.c_double()
+        check(self.lib.rtx_pupil_sum(self.ctx, N, A.ptr, P.ptr, None if w is None else w.ptr,
+                                     ptr(spec), U.ptr, C.byref(count), C.byref(sumw)))
+        return int(count.value), float(sumw.value)
+
+    def pupil_intensity(self, spec, U, psf, scale=1.0):
+        """rtx_pupil_intensity: ADD scale |U|^2 of the complex128 DeviceArray
+        U (K, nx, ny) to the float64 DeviceArray psf (K, nx, ny).  Returns the
+        stats (K, 5) of psf after the addition: sum, max, flat index of the
+        first max, sum psf p, sum psf q."""
+        spec = np.ascontiguousarray(spec, PUPIL_DTYPE).reshape(1)
+        s = spec[0]
+        K, need = int(s["planes"]), int(s["planes"])*int(s["nx"])*int(s["ny"])
+        if np.dtype(U.dtype) != np.complex128 or U.nbytes//16 < need:
+            raise ValueError("U must be a complex128 device array of %d values" % need)
+        if np.dtype(psf.dtype) != np.float64 or psf.nbytes//8 < need:
+            raise ValueError("psf must be a float64 device array of %d values" % need)
+        stats = np.zeros((max(K, 1), 5))
+        check(self.lib.rtx_pupil_intensity(self.ctx, ptr(spec), U.ptr, float(scale), psf.ptr,
+                                           ptr(stats)))
+        return stats
 
     # ---- lens-parameter derivatives --------------------------------------
     def trace_jacobian(self, table, y0, u0, moves, clip=False, rot0=None, exact=False, N=None):

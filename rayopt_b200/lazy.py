@@ -581,6 +581,83 @@ class ResidentMixin:
                                     **kwargs)
         return psf_profiles(self._engine(), p, out, self.psf_stats)
 
+    # ---- diffraction PSF by direct summation over the traced rays
+    def psf_direct(self, pixels=(128, 128), pitch=None, center=(0., 0.), defocus=(0.,),
+                   radius=None, after=-2, image=-1, weights=None, download=True):
+        """The diffraction PSF as the Debye sum of the pupil function over the
+        traced rays themselves (rtx_trace_opd, rtx_pupil_sum,
+        rtx_pupil_intensity): no regridding and no FFT, so obscured or
+        vignetted pupils keep their shape, and the grid is the caller's.  The
+        image grid is ``center + (a - nx//2) pitch`` along x and likewise
+        along y about the ref ray's image point (``pitch=None``: an eighth
+        of the Airy radius at the trace's wavelength), at each `defocus`
+        plane; the sphere is ``psf()``'s (``radius=None``:
+        ``system[-1].distance``).  `weights` (N,) per ray, numpy or a
+        DeviceArray (None: all 1).  Returns (p, q, psf (K, nx, ny)) in
+        Strehl units, |U|^2/(sum w)^2, psf a DeviceArray when not
+        `download` (free it when done).  ``self.psf_direct_stats`` holds
+        count (rays summed), left_out, sum_w, and per plane strehl (at the
+        chief point), peak, peak_at (p, q), centroid (p, q) and sum."""
+        from .engine import pupil_spec
+        eng = self._engine()
+        after, image = range(self.length)[after], range(self.length)[image]
+        radius = self.system[-1].distance if radius is None else float(radius)
+        nx, ny = (int(v) for v in pixels)
+        z = np.atleast_1d(np.asarray(defocus, np.float64))
+        lam = self.l/self.system.scale
+        if pitch is None:
+            par = self.system.paraxial
+            pitch = par.airy_radius[1]/par.wavelength*self.l/8
+        p = float(center[0]) + (np.arange(nx) - nx//2)*float(pitch)
+        q = float(center[1]) + (np.arange(ny) - ny//2)*float(pitch)
+        p0, q0 = float(center[0]) - (nx//2)*float(pitch), float(center[1]) - (ny//2)*float(pitch)
+        pupil_spec(z, (nx, ny), p0, pitch, q0, pitch, 0., lam, 1/lam, radius)   # refuse early
+        A, P = self._trace_opd(radius, after, image)
+        bufs = [A, P]
+        try:
+            ref = int(self.ref)
+            a0 = float(A.rows(ref).download()[0])
+            kappa = self.n[after]/lam
+            spec = pupil_spec(z, (nx, ny), p0, pitch, q0, pitch, a0, lam, kappa, radius)
+            chief = pupil_spec(z, (1, 1), 0., pitch, 0., pitch, a0, lam, kappa, radius)
+            w = weights
+            if w is not None and not hasattr(w, "ptr"):
+                w = eng.to_device(np.asarray(w, np.float64))
+                bufs.append(w)
+            U = eng.empty((len(z), nx, ny), np.complex128)
+            U1 = eng.empty((len(z), 1, 1), np.complex128)
+            bufs += [U, U1]
+            eng.memset(U)
+            eng.memset(U1)
+            count, sw = eng.pupil_sum(A, P, spec, U, w=w, N=self.nrays)
+            eng.pupil_sum(A, P, chief, U1, w=w, N=self.nrays)
+            if not count or not sw:
+                raise ValueError("no rays made it through")
+            out = eng.empty((len(z), nx, ny))
+            eng.memset(out)
+            try:
+                st = eng.pupil_intensity(spec, U, out, 1/sw**2)
+            except Exception:
+                out.free()
+                raise
+            u1 = U1.download()[:, 0, 0]
+        finally:
+            for a in bufs:
+                a.free()
+        at = st[:, 2].astype(np.int64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            self.psf_direct_stats = dict(
+                count=count, left_out=self.nrays - count, sum_w=sw,
+                strehl=np.abs(u1)**2/sw**2, peak=st[:, 1].copy(),
+                peak_at=np.stack([p[at//ny], q[at % ny]], -1), sum=st[:, 0].copy(),
+                centroid=st[:, 3:5]/st[:, :1])
+        pp, qq = np.broadcast_arrays(p[:, None], q[None, :])
+        if download:
+            psf = out.download()
+            out.free()
+            return pp, qq, psf
+        return pp, qq, out
+
     # ---- through-focus spot images (Analysis.spots, rayopt/analysis.py:250-283)
     def spot_image(self, defocus=(0.,), bins=(256, 256), range=None, at=-1, radial=False,
                    offsets=None, download=True):
