@@ -776,6 +776,64 @@ int rtx_otf_jacobian_sums(rtx_ctx *ctx, int64_t N, int P, const void *q, int qst
                           const void *J, int64_t ld, const double *center, int nfreq,
                           const double *freqs, double *out);
 
+/* ---- tolerance analysis on the geometric OTF ----------------------------- */
+/*
+ * The geometric OTF sums of many (surface table, launch bundle) items in ONE
+ * launch -- the MTF of thousands of perturbed lenses.  tables, S, rot0,
+ * dtype, nb, N, y0, u0, nitems, item_table, item_bundle and clip are
+ * rtx_trace_reduce_many's; item i is centred on centers[2i .. 2i+1] (host
+ * (nitems, 2), or NULL for 0).  Every item shares the planes z (host, K =
+ * planes values) and the frequencies freqs (host, F = nfreq values nu_j in
+ * cycles per length unit, any order: rtx_otf_jacobian_sums' convention).
+ * Each ray's state at surface S-1 is the last row rtx_trace stores for the
+ * same table, in every mode, and its point at plane k is rtx_otf_rows' with
+ * no offset (FP64, every operation separately rounded, FP32 rays widened
+ * first):
+ *   d = y_xy - c,  u = i_xy / i_z,  q_k = d + z[k] u
+ * A ray counts at plane k iff both components of q_k are finite (so a ray
+ * with i_z = 0 counts at no plane, not even at z = 0).  For a in {x, y}:
+ *   S[k,a,j] = sum over the counted rays of exp(-2 pi i nu_j q_k[a])
+ *   count[k] = number of counted rays;  OTF = S / count,  MTF = |OTF|
+ * with one sincospi(2 fl(nu_j q_k[a])) per term.  sums: host (nitems, K, 2,
+ * F, 2) doubles (re, im), count: host (nitems, K) int64; exactly
+ * nitems*K*2*F*2 doubles and nitems*K counts are written, zeros for N = 0.
+ *
+ * Deterministic: in each 512-ray tile of an item the rays are staged in
+ * shared memory; for each (plane, axis, frequency) unit lane l adds the
+ * terms of rays l, l + 32, .., l + 480 in that order, the 32 lanes are added
+ * by a shuffle tree, and the tile's sums go to its own row in the context.
+ * A second kernel adds each item's rows in tile order (no atomics).  So an
+ * item gives the same bits in every call and context, whatever the grid and
+ * whatever other items share the launch, in any order.
+ *
+ * Error bound against the exact sums of the same q_k, eps = 2^-52,
+ * Phi = max |nu_j q_k[a]| over the counted rays:
+ *   |S - S_exact| <= (D + 4 Phi + 3) eps count[k]   per component
+ *   D = 20 + ceil(N / 512)   (the summation depth)
+ * D bounds the additions: 15 in a lane, 5 in the shuffle tree and
+ * ceil(N/512) - 1 over the tiles, each partial sum's components at most the
+ * sum of the terms' magnitudes; 4 Phi the rounding of nu q, which moves the
+ * phase by at most pi Phi eps; 3 the 2 ulp of each sincospi component and
+ * one more.  Counts are exact.
+ *
+ * RTX_E_BADARG, before any device work or allocation: every refusal of
+ * rtx_trace_reduce_many (with sums and count in place of m); planes outside
+ * 1..RTX_OTF_MAX_PLANES or nfreq outside 1..RTX_OTF_MAX_FREQS; a NULL z,
+ * freqs, sums or count; a non-finite z, frequency or centre.  RTX_E_UNSUPPORTED
+ * as rtx_trace_reduce_many.  The device tables, the items and the tile rows
+ * ((K*2*F*2 + K) doubles per tile) are kept in the context: RTX_E_NOMEM
+ * before allocating when they do not fit.  Synchronous; rtx_last_kernel_ms
+ * covers the two kernels.
+ */
+int rtx_trace_otf_many(rtx_ctx *ctx, int nt, const rtx_surface *tables, int S,
+                       const double *rot0, int dtype, int nb, const int64_t *N,
+                       const void *const *y0, const void *const *u0,
+                       int64_t nitems, const int32_t *item_table,
+                       const int32_t *item_bundle, const double *centers,
+                       int clip, int planes, const double *z, int nfreq,
+                       const double *freqs, double *sums, int64_t *count,
+                       unsigned flags);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

@@ -1618,7 +1618,9 @@ template <typename T, int MODE>
 int launch_epi_kernel(rtx_ctx* ctx, unsigned flags, long long tiles, const EpiParams<T>& p) {
     constexpr int RPT = 2, threads = 256;
     static_assert(threads * RPT == EPI_TILE, "epi_kernel's tile");
-    size_t smem = (((size_t)p.S * sizeof(DevSurf<T>) + 127) & ~size_t(127)) + 16;
+    // the table, its barrier and (EPI_OTF) the tile's staged rays
+    size_t smem = (((size_t)p.S * sizeof(DevSurf<T>) + 127) & ~size_t(127)) +
+                  (MODE == EPI_OTF ? 128 + 4 * EPI_TILE * sizeof(double) : 16);
     if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
     auto go = [&](auto kern) -> int {
         if (smem > 48 * 1024)
@@ -1708,11 +1710,17 @@ int rtx_trace_reduce(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
 }  // extern "C"
 
 namespace {
-template <typename T>
-int trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
-                      const int64_t* N, const void* const* y0, const void* const* u0,
-                      long long nitems, const int32_t* item_table, const int32_t* item_bundle,
-                      const double* centers, int clip, double* m, unsigned flags) {
+// rtx_trace_reduce_many (MODE EPI_MANY, W = RTX_NMOMENTS, centres of 4
+// doubles) and rtx_trace_otf_many (EPI_OTF, W its row width, centres of 2):
+// the launch-wide tile list, the epilogue kernel over it, then the second
+// pass that adds each item's W-wide tile rows in tile order into out (host,
+// (nitems, W)).  `consts` go to the device after the items (EPI_OTF: z, nu).
+template <typename T, int MODE>
+int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
+               const int64_t* N, const void* const* y0, const void* const* u0, long long nitems,
+               const int32_t* item_table, const int32_t* item_bundle, const double* centers,
+               int cstride, int clip, int W, const std::vector<double>& consts, double* out,
+               unsigned flags, EpiParams<T>& p) {
     // the launch-wide tile list: item i owns tiles tile0 .. tile0 + ceil(N/512) - 1
     std::vector<EpiItem> items((size_t)nitems);
     long long tiles = 0;
@@ -1725,35 +1733,39 @@ int trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, co
         it.tile0 = tiles;
         it.table = item_table[i];
         for (int k = 0; k < 2; ++k) {
-            it.cy[k] = centers ? centers[4 * i + k] : 0.0;
-            it.cu[k] = centers ? centers[4 * i + 2 + k] : 0.0;
+            it.cy[k] = centers ? centers[cstride * i + k] : 0.0;
+            it.cu[k] = centers && cstride == 4 ? centers[cstride * i + 2 + k] : 0.0;
         }
         tiles += (N[b] + EPI_TILE - 1) / EPI_TILE;
     }
-    // one workspace: tables | items | tile sums | moments
+    // one workspace: tables | items | consts | tile rows | item rows
     auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t tb = up((size_t)nt * S * sizeof(DevSurf<T>)), ib = up(items.size() * sizeof(EpiItem));
-    const size_t mb = (size_t)nitems * RTX_NMOMENTS * sizeof(double);
-    if ((unsigned long long)tiles > (SIZE_MAX - tb - ib - mb) / (RTX_NMOMENTS * sizeof(double) + 1))
-        return RTX_E_NOMEM;
-    const size_t pb = up((size_t)tiles * RTX_NMOMENTS * sizeof(double));
+    const size_t cb = up(consts.size() * sizeof(double));
+    const size_t row = (size_t)W * sizeof(double);
+    if ((unsigned long long)nitems > (SIZE_MAX - tb - ib - cb) / (2 * row)) return RTX_E_NOMEM;
+    const size_t mb = (size_t)nitems * row;
+    if ((unsigned long long)tiles > (SIZE_MAX - tb - ib - cb - mb) / (row + 1)) return RTX_E_NOMEM;
+    const size_t pb = up((size_t)tiles * row);
     CK(cudaSetDevice(ctx->device));
     Workspace& ws = ctx->ws[WS_MANY];
-    int rc = reserve(ws, tb + ib + pb + mb);
+    int rc = reserve(ws, tb + ib + cb + pb + mb);
     if (rc) return rc;
     unsigned char* base = (unsigned char*)ws.p;
     DevSurf<T>* dtab = (DevSurf<T>*)base;
     EpiItem* ditems = (EpiItem*)(base + tb);
-    double* part = (double*)(base + tb + ib);
-    double* dm = (double*)(base + tb + ib + pb);
+    double* dconsts = (double*)(base + tb + ib);
+    double* part = (double*)(base + tb + ib + cb);
+    double* dm = (double*)(base + tb + ib + cb + pb);
     std::vector<DevSurf<T>> host((size_t)nt * S);
     for (size_t r = 0; r < host.size(); ++r) convert_surface<T>(tables[r], host[r]);
     CK(cudaMemcpyAsync(dtab, host.data(), host.size() * sizeof(DevSurf<T>), cudaMemcpyHostToDevice,
                        ctx->stream));
     CK(cudaMemcpyAsync(ditems, items.data(), items.size() * sizeof(EpiItem),
                        cudaMemcpyHostToDevice, ctx->stream));
-    EpiParams<T> p;
-    memset(&p, 0, sizeof(p));
+    if (!consts.empty())
+        CK(cudaMemcpyAsync(dconsts, consts.data(), consts.size() * sizeof(double),
+                           cudaMemcpyHostToDevice, ctx->stream));
     p.table = dtab;
     p.S = S;
     p.clip = clip ? 1 : 0;
@@ -1764,32 +1776,32 @@ int trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, co
     p.nitems = nitems;
     p.tiles = tiles;
     p.part = part;
+    p.otf_zf = dconsts;
     rc = timed(ctx, [&]() -> int {
         if (tiles > 0) {
-            int rc = launch_epi_kernel<T, EPI_MANY>(ctx, flags, tiles, p);
+            int rc = launch_epi_kernel<T, MODE>(ctx, flags, tiles, p);
             if (rc) return rc;
         }
-        many_sum_kernel<<<cap_grid(ctx, (nitems * RTX_NMOMENTS + 255) / 256, 8), 256, 0,
-                          ctx->stream>>>(ditems, nitems, part, dm);
+        if constexpr (MODE == EPI_MANY)
+            many_sum_kernel<<<cap_grid(ctx, (nitems * RTX_NMOMENTS + 255) / 256, 8), 256, 0,
+                              ctx->stream>>>(ditems, nitems, part, dm);
+        else
+            many_rows_kernel<<<cap_grid(ctx, (nitems * W + 255) / 256, 8), 256, 0, ctx->stream>>>(
+                ditems, nitems, W, part, dm);
         ctx->launches++;
         return (int)cudaGetLastError();
     });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(m, dm, mb, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out, dm, mb, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
-}  // namespace
 
-extern "C" {
-
-int rtx_trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S,
-                          const double* rot0, int dtype, int nb, const int64_t* N,
-                          const void* const* y0, const void* const* u0, int64_t nitems,
-                          const int32_t* item_table, const int32_t* item_bundle,
-                          const double* centers, int clip, double* m, unsigned flags) {
-    if (!ctx || !tables || !N || !y0 || !u0 || !item_table || !item_bundle || !m)
-        return RTX_E_BADARG;
+// the refusals rtx_trace_reduce_many and rtx_trace_otf_many share
+int check_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, int nb, const int64_t* N,
+               const void* const* y0, const void* const* u0, int64_t nitems,
+               const int32_t* item_table, const int32_t* item_bundle) {
+    if (!ctx || !tables || !N || !y0 || !u0 || !item_table || !item_bundle) return RTX_E_BADARG;
     if (nt < 1 || nb < 1 || nitems < 1 || S < 1 || S > RTX_MAX_SURFACES) return RTX_E_BADARG;
     for (int t = 0; t < nt; ++t) {
         int rc = check_table(tables + (size_t)t * S, S);
@@ -1801,11 +1813,68 @@ int rtx_trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S
         if (item_table[i] < 0 || item_table[i] >= nt || item_bundle[i] < 0 ||
             item_bundle[i] >= nb)
             return RTX_E_BADARG;
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_reduce_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S,
+                          const double* rot0, int dtype, int nb, const int64_t* N,
+                          const void* const* y0, const void* const* u0, int64_t nitems,
+                          const int32_t* item_table, const int32_t* item_bundle,
+                          const double* centers, int clip, double* m, unsigned flags) {
+    if (!m) return RTX_E_BADARG;
+    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
+    if (rc) return rc;
     return dispatch(dtype, [&](auto t) -> int {
         using T = decltype(t);
         if ((flags & RTX_EXACT) && sizeof(T) == 4) return RTX_E_UNSUPPORTED;
-        return trace_reduce_many<T>(ctx, nt, tables, S, rot0, N, y0, u0, nitems, item_table,
-                                    item_bundle, centers, clip, m, flags);
+        EpiParams<T> p;
+        memset(&p, 0, sizeof(p));
+        return trace_many<T, EPI_MANY>(ctx, nt, tables, S, rot0, N, y0, u0, nitems, item_table,
+                                       item_bundle, centers, 4, clip, RTX_NMOMENTS, {}, m, flags,
+                                       p);
+    });
+}
+
+int rtx_trace_otf_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
+                       int dtype, int nb, const int64_t* N, const void* const* y0,
+                       const void* const* u0, int64_t nitems, const int32_t* item_table,
+                       const int32_t* item_bundle, const double* centers, int clip, int planes,
+                       const double* z, int nfreq, const double* freqs, double* sums,
+                       int64_t* count, unsigned flags) {
+    if (!sums || !count || !z || !freqs) return RTX_E_BADARG;
+    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
+    if (rc) return rc;
+    if (planes < 1 || planes > RTX_OTF_MAX_PLANES || nfreq < 1 || nfreq > RTX_OTF_MAX_FREQS)
+        return RTX_E_BADARG;
+    const int K = planes, F = nfreq, W = 4 * K * F + K;
+    std::vector<double> consts(z, z + K);
+    consts.insert(consts.end(), freqs, freqs + F);
+    bool finite = true;
+    for (double v : consts) finite = finite && std::isfinite(v);
+    for (long long i = 0; centers && i < 2 * nitems; ++i) finite = finite && std::isfinite(centers[i]);
+    if (!finite) return RTX_E_BADARG;
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        if ((flags & RTX_EXACT) && sizeof(T) == 4) return RTX_E_UNSUPPORTED;
+        EpiParams<T> p;
+        memset(&p, 0, sizeof(p));
+        p.otf_K = K;
+        p.otf_F = F;
+        p.otf_W = W;
+        std::vector<double> rows((size_t)nitems * W);
+        int rc = trace_many<T, EPI_OTF>(ctx, nt, tables, S, rot0, N, y0, u0, nitems, item_table,
+                                        item_bundle, centers, 2, clip, W, consts, rows.data(),
+                                        flags, p);
+        if (rc) return rc;
+        for (long long i = 0; i < nitems; ++i) {
+            const double* r = rows.data() + (size_t)i * W;
+            memcpy(sums + (size_t)i * 4 * K * F, r, (size_t)4 * K * F * sizeof(double));
+            for (int k = 0; k < K; ++k) count[(size_t)i * K + k] = (int64_t)r[4 * K * F + k];
+        }
+        return 0;
     });
 }
 

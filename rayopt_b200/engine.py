@@ -695,13 +695,10 @@ class Engine:
             *args, None if w is None else w.ptr, ptr(c), ptr(m), self._flags(exact, False)))
         return m
 
-    def trace_reduce_many(self, tables, bundles, items, centers=None, clip=False, rot0=None,
-                          exact=False):
-        """rtx_trace_reduce_many: `tables` (nt, S) records, `bundles` a list
-        of (y0, u0, N) DEVICE launch rays (N None: all rows), `items` (nitems,
-        2) of (table, bundle) indices, `centers` (nitems, 4) guess centres or
-        None.  Returns the (nitems, 20) moments of every item (w = 1) from one
-        launch; each row's bits depend on its own item only."""
+    @staticmethod
+    def _many_args(tables, bundles, items):
+        """the checked arguments trace_reduce_many and trace_otf_many share:
+        (tables, dtype, items, N, y0s, u0s, item tables, item bundles)"""
         tables = np.ascontiguousarray(tables, SURFACE_DTYPE)
         if tables.ndim != 2 or tables.shape[0] < 1 or tables.shape[1] < 1:
             raise ValueError("tables must be a non-empty (nt, S) record array")
@@ -720,20 +717,59 @@ class Engine:
             raise ValueError("no items")
         if items.min() < 0 or items[:, 0].max() >= len(tables) or items[:, 1].max() >= len(bundles):
             raise ValueError("an item's table or bundle index is out of range")
-        c = None
-        if centers is not None:
-            c = np.ascontiguousarray(centers, np.float64).reshape(len(items), 4)
         it = np.ascontiguousarray(items[:, 0], np.int32)
         ib = np.ascontiguousarray(items[:, 1], np.int32)
         N = np.ascontiguousarray(Ns, np.int64)
         y0s = (C.c_void_p*len(bundles))(*[b[0].ptr for b in bundles])
         u0s = (C.c_void_p*len(bundles))(*[b[1].ptr for b in bundles])
+        return tables, dtype, items, N, y0s, u0s, it, ib
+
+    def trace_reduce_many(self, tables, bundles, items, centers=None, clip=False, rot0=None,
+                          exact=False):
+        """rtx_trace_reduce_many: `tables` (nt, S) records, `bundles` a list
+        of (y0, u0, N) DEVICE launch rays (N None: all rows), `items` (nitems,
+        2) of (table, bundle) indices, `centers` (nitems, 4) guess centres or
+        None.  Returns the (nitems, 20) moments of every item (w = 1) from one
+        launch; each row's bits depend on its own item only."""
+        tables, dtype, items, N, y0s, u0s, it, ib = self._many_args(tables, bundles, items)
+        c = None
+        if centers is not None:
+            c = np.ascontiguousarray(centers, np.float64).reshape(len(items), 4)
         m = np.zeros((len(items), 20))
         check(self.lib.rtx_trace_reduce_many(
             self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
             len(bundles), ptr(N), y0s, u0s, len(items), ptr(it), ptr(ib), ptr(c), int(bool(clip)),
             ptr(m), self._flags(exact, False)))
         return m
+
+    def trace_otf_many(self, tables, bundles, items, centers=None, z=(0.,), freqs=(0.,),
+                       clip=False, rot0=None, exact=False):
+        """rtx_trace_otf_many: `tables`, `bundles` and `items` as
+        trace_reduce_many, `centers` (nitems, 2) or None, the planes `z` (K,)
+        and the frequencies `freqs` (F,) every item shares.  Returns the
+        complex OTF sums (nitems, K, 2, F) (axis 0: x, 1: y) and the counts
+        (nitems, K) int64 from one launch; each item's bits depend on its own
+        item only."""
+        tables, dtype, items, N, y0s, u0s, it, ib = self._many_args(tables, bundles, items)
+        z = np.ascontiguousarray(np.atleast_1d(np.asarray(z, np.float64)))
+        nu = np.ascontiguousarray(np.atleast_1d(np.asarray(freqs, np.float64)))
+        K, F = len(z), len(nu)
+        if z.ndim != 1 or not 1 <= K <= OTF_MAX_PLANES or not np.isfinite(z).all():
+            raise ValueError("need 1..%d finite planes, got %r" % (OTF_MAX_PLANES, z))
+        if nu.ndim != 1 or not 1 <= F <= OTF_MAX_FREQS or not np.isfinite(nu).all():
+            raise ValueError("need 1..%d finite frequencies, got %r" % (OTF_MAX_FREQS, nu))
+        c = None
+        if centers is not None:
+            c = np.ascontiguousarray(centers, np.float64).reshape(len(items), 2)
+            if not np.isfinite(c).all():
+                raise ValueError("centres must be finite")
+        sums = np.zeros((len(items), K, 2, F, 2))
+        count = np.zeros((len(items), K), np.int64)
+        check(self.lib.rtx_trace_otf_many(
+            self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
+            len(bundles), ptr(N), y0s, u0s, len(items), ptr(it), ptr(ib), ptr(c), int(bool(clip)),
+            K, ptr(z), F, ptr(nu), ptr(sums), ptr(count), self._flags(exact, False)))
+        return sums[..., 0] + 1j*sums[..., 1], count
 
     @staticmethod
     def rms_finite_from_moments(m):

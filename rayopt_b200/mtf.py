@@ -9,7 +9,7 @@ defocus plane about a centre, along x (sagittal for fields along y) or y
 """
 import numpy as np
 
-from .engine import default_engine, otf_spec
+from .engine import OTF_MAX_FREQS, default_engine, otf_spec
 
 
 def _otf(S, count):
@@ -124,3 +124,19 @@ def poly_otf(otf, count, weights):
     num = np.einsum("hwk,hwkaf->hkaf", wk, np.where(wk[..., None, None] > 0, otf, 0))
     with np.errstate(invalid="ignore", divide="ignore"):
         return num/wk.sum(1)[..., None, None]
+
+
+def _check_freqs(freqs):
+    nu = np.ascontiguousarray(np.atleast_1d(np.asarray(freqs, np.float64)))
+    if nu.ndim != 1 or not 1 <= len(nu) <= OTF_MAX_FREQS or not np.isfinite(nu).all():
+        raise ValueError("need 1..%d finite frequencies, got %r" % (OTF_MAX_FREQS, freqs))
+    return nu
+
+
+def _spectral(spectral_weights, W):
+    if spectral_weights is None:
+        return np.ones(W)
+    sw = np.asarray(spectral_weights, np.float64)
+    if sw.size != W or not np.isfinite(sw).all():
+        raise ValueError("spectral_weights must be %d finite values, got %r" % (W, spectral_weights))
+    return sw.reshape(W)

@@ -47,10 +47,10 @@ import copy
 
 import numpy as np
 
-from .engine import (OTF_MAX_FREQS, Engine, default_engine, jacobian_sums_unpack,
-                     otf_jacobian_sums_unpack, wavefront_sums_unpack)
+from .engine import (Engine, default_engine, jacobian_sums_unpack, otf_jacobian_sums_unpack,
+                     wavefront_sums_unpack)
 from .lazy import opd_spec
-from .mtf import poly_otf
+from .mtf import _check_freqs, _spectral, poly_otf
 from .surface_table import RTX_MAX_ASPH, SURFACE_DTYPE, pack_system
 from .tolerance import _chief, launch_bundles, perturbed_tables, record_tangents
 
@@ -617,22 +617,6 @@ def optimize_wavefront(system, params, heights=(0., .707, 1.), wavelengths=None,
 
 
 # ---- the geometric MTF at chosen frequencies -------------------------------
-def _check_freqs(freqs):
-    nu = np.ascontiguousarray(np.atleast_1d(np.asarray(freqs, np.float64)))
-    if nu.ndim != 1 or not 1 <= len(nu) <= OTF_MAX_FREQS or not np.isfinite(nu).all():
-        raise ValueError("need 1..%d finite frequencies, got %r" % (OTF_MAX_FREQS, freqs))
-    return nu
-
-
-def _spectral(spectral_weights, W):
-    if spectral_weights is None:
-        return np.ones(W)
-    sw = np.asarray(spectral_weights, np.float64)
-    if sw.size != W or not np.isfinite(sw).all():
-        raise ValueError("spectral_weights must be %d finite values, got %r" % (W, spectral_weights))
-    return sw.reshape(W)
-
-
 def _per_residual(name, x, shape):
     """`x` broadcast to (H, 2, F), ValueError when it does not"""
     try:

@@ -304,9 +304,35 @@ def focus_shifts(m, weights):
                     ).reshape(tot.shape[:-1])
 
 
-def _variant_chunk(tables_bytes_per_variant, tiles_per_variant, budget):
-    per = tables_bytes_per_variant + 160*tiles_per_variant + 1
+def _variant_chunk(tables_bytes_per_variant, tiles_per_variant, budget, row_bytes=160,
+                   items_per_variant=0):
+    """variants per launch whose device tables, tile rows and item rows
+    (`row_bytes` each: 20 moments, or an OTF row) fit in `budget` bytes"""
+    per = tables_bytes_per_variant + row_bytes*(tiles_per_variant + items_per_variant) + 1
     return max(1, int(budget//per))
+
+
+def _focus(eng, fsys, nominal, params, deltas, l, rot0, step, exact):
+    """(V,) GeometricTrace.refocus's shift of every variant: 13 Radau rays
+    on axis at `l`, unclipped, aimed on `fsys` (the NOMINAL lens), marched
+    through each variant's table at `l` (nominal[0]), `step` variants per
+    launch"""
+    fb = _focus_bundles(fsys, l, eng)
+    try:
+        G, V = len(fb), len(deltas)
+        focus = np.empty(V)
+        for v0 in range(0, V, step):
+            t = perturbed_tables(nominal[:1], params, deltas[v0:v0 + step])[:, 0]
+            n = len(t)
+            items = np.stack(np.meshgrid(np.arange(n), np.arange(G), indexing="ij"),
+                             -1).reshape(-1, 2)
+            m = eng.trace_reduce_many(t, [(y, u, None) for _, y, u in fb], items,
+                                      clip=False, rot0=rot0, exact=exact)
+            focus[v0:v0 + n] = focus_shifts(m.reshape(n, G, 20), [w for w, _, _ in fb])
+    finally:
+        for _, y, u in fb:
+            y.free(), u.free()
+    return focus
 
 
 def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, nrays=1000,
@@ -348,7 +374,7 @@ def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, 
     # bundle is aimed on a copy taken before any
     fsys = copy.deepcopy(system) if compensate == "focus" else None
     bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    focus = fb = None
+    focus = None
     try:
         centers = np.array([_chief(eng, nominal[b % W], rot0, y, u, exact)
                             for b, (y, u) in enumerate(chiefs)])
@@ -359,17 +385,7 @@ def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, 
         if step < 1:
             raise ValueError("chunk must be >= 1")
         if compensate == "focus":
-            fb = _focus_bundles(fsys, wavelengths[0], eng)
-            G = len(fb)
-            focus = np.empty(V)
-            for v0 in range(0, V, step):
-                t = perturbed_tables(nominal[:1], params, deltas[v0:v0 + step])[:, 0]
-                n = len(t)
-                items = np.stack(np.meshgrid(np.arange(n), np.arange(G), indexing="ij"),
-                                 -1).reshape(-1, 2)
-                m = eng.trace_reduce_many(t, [(y, u, None) for _, y, u in fb], items,
-                                          clip=False, rot0=rot0, exact=exact)
-                focus[v0:v0 + n] = focus_shifts(m.reshape(n, G, 20), [w for w, _, _ in fb])
+            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
         moments = np.empty((V, H, W, 20))
         vv, hh, ww = np.meshgrid(np.arange(V), np.arange(H), np.arange(W), indexing="ij")
         for v0 in range(0, V, step):
@@ -387,8 +403,6 @@ def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, 
     finally:
         for y, u in bundles:
             y.free(), u.free()
-        for _, y, u in fb or ():
-            y.free(), u.free()
     m = moments
     with np.errstate(all="ignore"):
         out = dict(rms=Engine.rms_finite_from_moments(m), transmitted=m[..., 4]/m[..., 5],
@@ -396,6 +410,134 @@ def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, 
                    moments=m, heights=np.asarray(heights, np.float64),
                    wavelengths=np.asarray(wavelengths, np.float64), params=params,
                    deltas=deltas)
+    if focus is not None:
+        out["focus"] = focus
+    return out
+
+
+def _otf_targets(targets, shape):
+    """`targets` broadcast to (H, 2, F), ValueError when it does not"""
+    try:
+        return np.broadcast_to(np.asarray(targets, np.float64), shape)
+    except ValueError:
+        raise ValueError("targets of shape %s does not broadcast to (heights, 2, freqs) = %s"
+                         % (np.shape(targets), shape)) from None
+
+
+def mtf_tolerance_result(sums, count, weights, targets=None):
+    """tolerance_mtf's result from the OTF sums (V, H, W, K, 2, F) complex
+    and counts (V, H, W, K): otf = sums/count (NaN where nothing counted),
+    mtf, poly (V, H, K, 2, F) (mtf.poly_otf with the spectral `weights`)
+    and poly_mtf; with `targets` (broadcast to (H, 2, F)) passed (V, K),
+    true where every poly MTF of the plane is at or above its target (NaN
+    fails), and yield (K,) the fraction of variants that pass"""
+    from .mtf import _otf, poly_otf
+    sums = np.asarray(sums, np.complex128)
+    count = np.asarray(count, np.int64)
+    V, H, W, K, _, F = sums.shape
+    otf = _otf(sums, count)
+    poly = poly_otf(otf.reshape(V*H, W, K, 2, F), count.reshape(V*H, W, K),
+                    weights).reshape(V, H, K, 2, F)
+    out = dict(otf=otf, mtf=np.abs(otf), count=count, poly=poly, poly_mtf=np.abs(poly))
+    if targets is not None:
+        t = _otf_targets(targets, (H, 2, F))
+        with np.errstate(invalid="ignore"):
+            ok = out["poly_mtf"] >= t[:, None]
+        out["passed"] = ok.all(axis=(1, 3, 4))
+        out["yield"] = out["passed"].mean(0)
+    return out
+
+
+def tolerance_mtf(system, params, deltas, freqs, heights=(0., .707, 1.), wavelengths=None,
+                  nrays=1000, distribution="hexapolar", defocus=(0.,), compensate=None,
+                  spectral_weights=None, targets=None, engine=None, exact=False, chunk=None):
+    """Geometric OTF and MTF of every perturbed lens at the frequencies
+    `freqs` (cycles per length unit), every field height, wavelength and
+    defocus plane, on the device: the MTF counterpart of ``tolerance``.
+
+    `params` [(j, kind)] and `deltas` (V, P) are ``perturbed_tables``'.
+    Each (height, wavelength) bundle is aimed once for the NOMINAL lens and
+    marched through all V variants with clipping (no re-aiming); every
+    variant's bundles are reduced to their OTF sums in the same launch as
+    the march (rtx_trace_otf_many).  As in geometric_mtf, every wavelength
+    of a height is centred on the nominal chief ray at wavelengths[0]; the
+    MTF does not depend on the centre.  `defocus` are up to 16 plane
+    distances from the image surface.  ``compensate="focus"`` refocuses each
+    variant first, as ``tolerance`` does.  `targets` (broadcast to (H, 2,
+    F)) are the minimum polychromatic MTF of an accepted lens.  `chunk`:
+    variants per launch (default: as many as fit in 1 GiB of tables and tile
+    rows); the results do not depend on it.
+
+    Returns a dict: freq (F,), z (K,), otf complex (V, H, W, K, 2, F)
+    (axis 0: x, sagittal; 1: y, tangential), mtf = |otf|, count (V, H, W,
+    K), poly (V, H, K, 2, F) the `spectral_weights` mean of the
+    wavelengths' OTFs (mtf.poly_otf), poly_mtf = |poly|, focus (V,) when
+    compensated, heights, wavelengths, params, deltas; with `targets`
+    also passed (V, K) (every poly MTF of the plane at or above its target,
+    NaN failing) and yield (K,), the fraction of variants that pass.
+    Every argument is checked before any device work."""
+    from .engine import OTF_MAX_PLANES
+    from .mtf import _check_freqs, _spectral
+    from .surface_table import pack_system
+    if compensate not in (None, "focus"):
+        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    H, W = len(heights), len(wavelengths)
+    nu = _check_freqs(freqs)
+    z = np.atleast_1d(np.asarray(defocus, np.float64))
+    if z.ndim != 1 or not 1 <= len(z) <= OTF_MAX_PLANES or not np.isfinite(z).all():
+        raise ValueError("defocus must be 1..%d finite distances, got %r" % (OTF_MAX_PLANES, defocus))
+    F, K = len(nu), len(z)
+    sw = _spectral(spectral_weights, W)
+    if targets is not None:
+        targets = _otf_targets(targets, (H, 2, F))
+    if chunk is not None and int(chunk) < 1:
+        raise ValueError("chunk must be >= 1")
+    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
+    nominal = np.stack([t for t, _, _ in packs])
+    rot0 = packs[0][2]
+    S = nominal.shape[1]
+    params = list(params)
+    deltas = np.asarray(deltas, np.float64)
+    if deltas.ndim == 1:
+        deltas = deltas[None]
+    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
+    V = deltas.shape[0]
+    eng = engine or default_engine()
+    fsys = copy.deepcopy(system) if compensate == "focus" else None
+    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
+    focus = None
+    sums = np.empty((V, H, W, K, 2, F), np.complex128)
+    count = np.empty((V, H, W, K), np.int64)
+    try:
+        # the chief ray of each height at wavelengths[0], for every wavelength
+        centers = np.array([_chief(eng, nominal[0], rot0, *chiefs[h*W], exact)[:2]
+                            for h in range(H)])
+        dev = [(y, u, None) for y, u in bundles]
+        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
+        step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 8*(4*K*F + K), H*W)
+        if compensate == "focus":
+            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
+        vv, hh, ww = np.meshgrid(np.arange(V), np.arange(H), np.arange(W), indexing="ij")
+        for v0 in range(0, V, step):
+            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+            n = len(t)
+            if focus is not None:                              # system[-1].distance += shift
+                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
+                                                          focus[v0:v0 + n, None])
+            sl = slice(v0*H*W, (v0 + n)*H*W)
+            v, h, w = vv.reshape(-1)[sl] - v0, hh.reshape(-1)[sl], ww.reshape(-1)[sl]
+            s, c = eng.trace_otf_many(t.reshape(n*W, S), dev, np.stack([v*W + w, h*W + w], -1),
+                                      centers[h], z, nu, clip=True, rot0=rot0, exact=exact)
+            sums[v0:v0 + n] = s.reshape(n, H, W, K, 2, F)
+            count[v0:v0 + n] = c.reshape(n, H, W, K)
+    finally:
+        for y, u in bundles:
+            y.free(), u.free()
+    out = mtf_tolerance_result(sums, count, sw, targets)
+    out.update(freq=nu, z=z, heights=np.asarray(heights, np.float64),
+               wavelengths=np.asarray(wavelengths, np.float64), params=params, deltas=deltas)
     if focus is not None:
         out["focus"] = focus
     return out
