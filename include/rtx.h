@@ -834,6 +834,57 @@ int rtx_trace_otf_many(rtx_ctx *ctx, int nt, const rtx_surface *tables, int S,
                        const double *freqs, double *sums, int64_t *count,
                        unsigned flags);
 
+/* ---- tolerance analysis on the rms wavefront ----------------------------- */
+/*
+ * rtx_trace_opd's per-ray path A and sphere point P of many (surface table,
+ * launch bundle) items in ONE launch, reduced to the sums of a least-squares
+ * fit of piston and tilt -- the rms wavefront of thousands of perturbed
+ * lenses.  tables, S, rot0, nb, N, y0, u0, nitems, item_table, item_bundle
+ * and clip are rtx_trace_reduce_many's; the tables are the march to `after`,
+ * as rtx_trace_opd's (surf[S] = system[1:after+1]: the image record is not
+ * marched).  Item i has its own sphere specs[i] (host, nitems records), its
+ * piston guess a0[i] (host, nitems doubles, or NULL for 0) and its pupil
+ * centre centers[2i .. 2i+1] (host (nitems, 2), or NULL for 0).
+ *
+ * Per ray, in FP64 with every operation separately rounded: A and P are the
+ * values rtx_trace_opd writes for the item's table and spec, bit for bit,
+ *   a = A - a0,  x = P_x - c_x,  y = P_y - c_y
+ * and the ray enters iff a, x and y are all finite.  sums: host (nitems,
+ * RTX_WFE_NSUMS), each row over the rays that enter, in this order:
+ *   n, sum a, sum a^2, sum x, sum y, sum x^2, sum xy, sum y^2, sum ax, sum ay
+ * zeros for N = 0; exactly nitems*RTX_WFE_NSUMS doubles are written.  With
+ * a0 = A[ref], c = P_xy[ref] the residuals are opd()'s chief-referenced t
+ * (times -l/scale) and py.
+ *
+ * Deterministic as rtx_trace_reduce_many: each 512-ray tile's sums (every
+ * product rounded once, then a lane's 2 rays, a shuffle tree, the 8 warps
+ * in order) go to the tile's own row, and a second kernel adds each item's
+ * rows in tile order (no atomics).  An item gives the same bits in every
+ * call and context, whatever other items share the launch, in any order.
+ * Error bound against the exact sums of the same a, x, y (the terms are
+ * the exact products), eps = 2^-52:
+ *   |sum - exact| <= (ceil(N/512) + 64) eps sum|term|   per sum
+ * (the summation depth is 12 + ceil(N/512) additions and one product
+ * rounding, each eps/2).  Counts are exact.
+ *
+ * FP64 only, fast or RTX_EXACT: RTX_F32 returns RTX_E_UNSUPPORTED (an FP32
+ * path sum of a ~100 mm track is worth about 0.02 waves).  RTX_E_BADARG,
+ * before any device work or allocation: every refusal of
+ * rtx_trace_reduce_many (with sums in place of m); a NULL specs; a
+ * non-finite a0, centre or spec member; a zero radius.  The device tables,
+ * the items, their specs and the tile rows (RTX_NMOMENTS doubles per tile)
+ * are kept in the context: RTX_E_NOMEM before allocating when they do not
+ * fit.  Synchronous; rtx_last_kernel_ms covers the two kernels.
+ */
+#define RTX_WFE_NSUMS 10
+int rtx_trace_opd_many(rtx_ctx *ctx, int nt, const rtx_surface *tables, int S,
+                       const double *rot0, int dtype, int nb, const int64_t *N,
+                       const void *const *y0, const void *const *u0,
+                       int64_t nitems, const int32_t *item_table,
+                       const int32_t *item_bundle, const rtx_opd *specs,
+                       const double *a0, const double *centers, int clip,
+                       double *sums, unsigned flags);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

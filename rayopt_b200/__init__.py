@@ -17,8 +17,9 @@ from .spot import spots  # noqa: F401
 from .opd import opds  # noqa: F401
 from .mtf import geometric_mtf  # noqa: F401
 from .psf import psfs  # noqa: F401
-from .tolerance import (tolerance, tolerance_mtf, perturbed_tables,  # noqa: F401
-                        sensitivity_deltas, monte_carlo_deltas, record_tangents)
+from .tolerance import (tolerance, tolerance_mtf, tolerance_wavefront,  # noqa: F401
+                        perturbed_tables, sensitivity_deltas, monte_carlo_deltas,
+                        record_tangents)
 from .optimize import (spot_jacobian, optimize_spot, wavefront_jacobian,  # noqa: F401
                        optimize_wavefront, mtf_jacobian, optimize_mtf)
 

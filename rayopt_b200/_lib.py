@@ -63,6 +63,8 @@ SYMBOLS = {
     "rtx_trace_reduce": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_reduce_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
                                    _vp, _i, _vp, _u]),
+    "rtx_trace_opd_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
+                                _vp, _vp, _vp, _i, _vp, _u]),
     "rtx_trace_otf_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
                                 _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_opd": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),

@@ -1711,10 +1711,12 @@ int rtx_trace_reduce(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
 
 namespace {
 // rtx_trace_reduce_many (MODE EPI_MANY, W = RTX_NMOMENTS, centres of 4
-// doubles) and rtx_trace_otf_many (EPI_OTF, W its row width, centres of 2):
-// the launch-wide tile list, the epilogue kernel over it, then the second
-// pass that adds each item's W-wide tile rows in tile order into out (host,
-// (nitems, W)).  `consts` go to the device after the items (EPI_OTF: z, nu).
+// doubles), rtx_trace_otf_many (EPI_OTF, W its row width, centres of 2) and
+// rtx_trace_opd_many (EPI_WFE, W = RTX_NMOMENTS, no centres): the launch-wide
+// tile list, the epilogue kernel over it, then the second pass that adds
+// each item's W-wide tile rows in tile order into out (host, (nitems, W)).
+// `consts` go to the device after the items (EPI_OTF: z, nu; EPI_WFE: the
+// WfeItem of every item).
 template <typename T, int MODE>
 int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
                const int64_t* N, const void* const* y0, const void* const* u0, long long nitems,
@@ -1777,12 +1779,13 @@ int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const dou
     p.tiles = tiles;
     p.part = part;
     p.otf_zf = dconsts;
+    if constexpr (MODE == EPI_WFE) p.wfe = reinterpret_cast<const WfeItem*>(dconsts);
     rc = timed(ctx, [&]() -> int {
         if (tiles > 0) {
             int rc = launch_epi_kernel<T, MODE>(ctx, flags, tiles, p);
             if (rc) return rc;
         }
-        if constexpr (MODE == EPI_MANY)
+        if constexpr (MODE == EPI_MANY || MODE == EPI_WFE)
             many_sum_kernel<<<cap_grid(ctx, (nitems * RTX_NMOMENTS + 255) / 256, 8), 256, 0,
                               ctx->stream>>>(ditems, nitems, part, dm);
         else
@@ -1797,7 +1800,8 @@ int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const dou
     return 0;
 }
 
-// the refusals rtx_trace_reduce_many and rtx_trace_otf_many share
+// the refusals rtx_trace_reduce_many, rtx_trace_otf_many and
+// rtx_trace_opd_many share
 int check_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, int nb, const int64_t* N,
                const void* const* y0, const void* const* u0, int64_t nitems,
                const int32_t* item_table, const int32_t* item_bundle) {
@@ -1875,6 +1879,59 @@ int rtx_trace_otf_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, c
             for (int k = 0; k < K; ++k) count[(size_t)i * K + k] = (int64_t)r[4 * K * F + k];
         }
         return 0;
+    });
+}
+
+int rtx_trace_opd_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
+                       int dtype, int nb, const int64_t* N, const void* const* y0,
+                       const void* const* u0, int64_t nitems, const int32_t* item_table,
+                       const int32_t* item_bundle, const rtx_opd* specs, const double* a0,
+                       const double* centers, int clip, double* sums, unsigned flags) {
+    static_assert(RTX_WFE_NSUMS == WFE_NSUMS && WFE_NSUMS <= RTX_NMOMENTS, "rtx_trace_opd_many's row");
+    if (!sums || !specs) return RTX_E_BADARG;
+    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
+    if (rc) return rc;
+    // every item's WfeItem, checked before any device work
+    std::vector<double> consts((size_t)nitems * WFE_ITEM_DOUBLES);
+    for (long long i = 0; i < nitems; ++i) {
+        const rtx_opd& o = specs[i];
+        WfeItem w;
+        for (int k = 0; k < 3; ++k) {
+            w.y0r[k] = o.y0_ref[k];
+            w.u0r[k] = o.u0_ref[k];
+            w.d[k] = o.d[k];
+        }
+        for (int k = 0; k < 9; ++k) w.M[k] = o.M[k];
+        w.n0 = o.n0;
+        w.n_after = o.n_after;
+        w.radius = o.radius;
+        w.infinite = o.infinite ? 1.0 : 0.0;
+        w.a0 = a0 ? a0[i] : 0.0;
+        w.c[0] = centers ? centers[2 * i] : 0.0;
+        w.c[1] = centers ? centers[2 * i + 1] : 0.0;
+        const double* v = reinterpret_cast<const double*>(&w);
+        for (int k = 0; k < WFE_ITEM_DOUBLES; ++k)
+            if (!std::isfinite(v[k])) return RTX_E_BADARG;
+        if (w.radius == 0.0) return RTX_E_BADARG;
+        memcpy(consts.data() + (size_t)i * WFE_ITEM_DOUBLES, &w, sizeof(w));
+    }
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        if constexpr (sizeof(T) != 8) {
+            return RTX_E_UNSUPPORTED;  // an FP32 path sum of a long track is worth ~0.02 waves
+        } else {
+            EpiParams<T> p;
+            memset(&p, 0, sizeof(p));
+            std::vector<double> rows((size_t)nitems * RTX_NMOMENTS);
+            int rc = trace_many<T, EPI_WFE>(ctx, nt, tables, S, rot0, N, y0, u0, nitems,
+                                            item_table, item_bundle, nullptr, 2, clip,
+                                            RTX_NMOMENTS, consts, rows.data(), flags, p);
+            if (rc) return rc;
+            for (long long i = 0; i < nitems; ++i)
+                memcpy(sums + (size_t)i * RTX_WFE_NSUMS, rows.data() + (size_t)i * RTX_NMOMENTS,
+                       RTX_WFE_NSUMS * sizeof(double));
+            return 0;
+        }
     });
 }
 

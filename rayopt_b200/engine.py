@@ -53,6 +53,7 @@ def spot_spec(z, bins, range, center, radial=False, offsets=None):
 
 # mirrors `struct rtx_otf` (include/rtx.h)
 OTF_MAX_PLANES, OTF_MAX_FREQS = 16, 256
+WFE_NSUMS = 10      # RTX_WFE_NSUMS: n, sum a, a^2, x, y, x^2, xy, y^2, ax, ay
 OTF_SLOT, OTF_BLOCK = 16384, 16      # RTX_OTF_SLOT, RTX_OTF_BLOCK
 MAX_PARAMS, JAC_SLOT = 64, 16384     # RTX_MAX_PARAMS, RTX_JAC_SLOT
 OTF_DTYPE = np.dtype([("planes", "<i4"), ("nfreq", "<i4"), ("dnu", "<f8"), ("c", "<f8", (2,)),
@@ -697,7 +698,8 @@ class Engine:
 
     @staticmethod
     def _many_args(tables, bundles, items):
-        """the checked arguments trace_reduce_many and trace_otf_many share:
+        """the checked arguments trace_reduce_many, trace_otf_many and
+        trace_opd_many share:
         (tables, dtype, items, N, y0s, u0s, item tables, item bundles)"""
         tables = np.ascontiguousarray(tables, SURFACE_DTYPE)
         if tables.ndim != 2 or tables.shape[0] < 1 or tables.shape[1] < 1:
@@ -770,6 +772,35 @@ class Engine:
             len(bundles), ptr(N), y0s, u0s, len(items), ptr(it), ptr(ib), ptr(c), int(bool(clip)),
             K, ptr(z), F, ptr(nu), ptr(sums), ptr(count), self._flags(exact, False)))
         return sums[..., 0] + 1j*sums[..., 1], count
+
+    def trace_opd_many(self, tables, bundles, items, specs, a0=None, centers=None, clip=False,
+                       rot0=None, exact=False):
+        """rtx_trace_opd_many: `tables` (nt, S) records of the march to
+        `after` (trace_opd's), `bundles` and `items` as trace_reduce_many,
+        `specs` one rtx_opd per item (a list of dicts with its members, or an
+        OPD_DTYPE array), `a0` (nitems,) piston guesses and `centers`
+        (nitems, 2) pupil centres, or None for 0.  Returns the (nitems, 10)
+        sums n, sum a, sum a^2, sum x, sum y, sum x^2, sum xy, sum y^2,
+        sum ax, sum ay of a = A - a0, (x, y) = P_xy - c over the rays whose
+        a, x, y are finite, from one launch; FP64 only; each row's bits
+        depend on its own item only."""
+        tables, dtype, items, N, y0s, u0s, it, ib = self._many_args(tables, bundles, items)
+        n = len(items)
+        if isinstance(specs, np.ndarray) and specs.dtype == OPD_DTYPE:
+            rec = np.ascontiguousarray(specs.reshape(-1))
+        else:
+            rec = np.concatenate([_opd_record(s) for s in specs]) if len(specs) else \
+                np.zeros(0, OPD_DTYPE)
+        if len(rec) != n:
+            raise ValueError("need one spec per item: %d specs for %d items" % (len(rec), n))
+        a = None if a0 is None else np.ascontiguousarray(a0, np.float64).reshape(n)
+        c = None if centers is None else np.ascontiguousarray(centers, np.float64).reshape(n, 2)
+        sums = np.zeros((n, WFE_NSUMS))
+        check(self.lib.rtx_trace_opd_many(
+            self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
+            len(bundles), ptr(N), y0s, u0s, n, ptr(it), ptr(ib), ptr(rec), ptr(a), ptr(c),
+            int(bool(clip)), ptr(sums), self._flags(exact, False)))
+        return sums
 
     @staticmethod
     def rms_finite_from_moments(m):

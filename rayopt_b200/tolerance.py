@@ -541,3 +541,241 @@ def tolerance_mtf(system, params, deltas, freqs, heights=(0., .707, 1.), wavelen
     if focus is not None:
         out["focus"] = focus
     return out
+
+
+# ---- the rms wavefront ------------------------------------------------------
+def wavefront_specs(base, tables, chief, Ri, origin0, image):
+    """The rtx_opd records (OPD_DTYPE, (n,)) of opd()'s reference sphere for
+    n variants of one wavelength, each centred on its own chief ray.
+
+    `base` the nominal lens's spec (lazy.opd_spec): its radius, launch ray
+    and n0 are kept.  `tables` (n, S) the variants' full tables (row S-1 the
+    image), `chief` (n, 2) each variant's chief-ray image point x, y (its z
+    is the sag of `image`, the nominal image record: the image surface's
+    shape is not perturbed), `Ri` the image surface's rot_normal and
+    `origin0` the object's offset.  Per variant, as opd_spec makes them from
+    a System with the same change: n_after = record S-2's n, M = rot(record
+    S-2) @ Ri.T (a tilt of the last lens surface turns it), and d =
+    (origins[after] - origins[image]) @ Ri.T - Y with the origins the
+    cumulative offsets."""
+    from .engine import OPD_DTYPE, _opd_record
+    from .optimize import _image_sag
+    tables = np.asarray(tables, SURFACE_DTYPE)
+    n, S = tables.shape
+    rec = np.repeat(_opd_record(base), n)
+    rec["n_after"] = tables[:, S - 2]["n"]
+    Ri = np.asarray(Ri, np.float64)
+    rec["M"] = (tables[:, S - 2]["rot"].reshape(n, 3, 3) @ Ri.T).reshape(n, 9)
+    off = np.concatenate([np.broadcast_to(np.asarray(origin0, np.float64), (n, 1, 3)),
+                          tables["offset"]], axis=1)
+    origins = np.cumsum(off, axis=1)                          # System.origins
+    chief = np.asarray(chief, np.float64).reshape(n, 2)
+    x, y = chief[:, 0], chief[:, 1]
+    Y = np.stack([x, y, _image_sag(image, x, y)], -1)
+    rec["d"] = (origins[:, S - 1] - origins[:, S]) @ Ri.T - Y
+    return rec.astype(OPD_DTYPE)
+
+
+def _tilt_fit(s):
+    """(SSR, Caa, n) of the least-squares fit of 1, x, y to a from the 10
+    sums s (..., 10) (rtx_trace_opd_many's order), formed from the centred
+    second moments in long double; a rank-deficient pupil (all points on
+    one line or one point) takes the minimum-norm fit.  SSR is clamped to
+    >= 0"""
+    s = np.asarray(s, np.longdouble)
+    n, sa, saa, sx, sy, sxx, sxy, syy, sax, say = np.moveaxis(s, -1, 0)
+    with np.errstate(all="ignore"):
+        ma, mx, my = sa/n, sx/n, sy/n
+        Caa = saa - sa*ma
+        Cxx, Cxy, Cyy = sxx - sx*mx, sxy - sx*my, syy - sy*my
+        Cax, Cay = sax - sx*ma, say - sy*ma
+        det = Cxx*Cyy - Cxy*Cxy
+        full = det > 1e-12*Cxx*Cyy
+        fit2 = (Cyy*Cax*Cax - 2*Cxy*Cax*Cay + Cxx*Cay*Cay)/det
+        lam = Cxx + Cyy                                       # rank 1: C = lam e e^T
+        fit1 = np.where(lam > 0, (Cxx*Cax*Cax + 2*Cxy*Cax*Cay + Cyy*Cay*Cay)/(lam*lam), 0)
+        ssr = Caa - np.where(full, fit2, fit1)
+        ssr = np.where(ssr < 0, 0, ssr)
+    return ssr, Caa, n
+
+
+def _wfe_targets(targets, H):
+    """`targets` broadcast to (H,), ValueError when it does not"""
+    try:
+        t = np.broadcast_to(np.asarray(targets, np.float64), (H,))
+    except ValueError:
+        raise ValueError("targets of shape %s does not broadcast to (heights,) = (%d,)"
+                         % (np.shape(targets), H)) from None
+    return t
+
+
+def wavefront_tolerance_result(sums, wl, N, weights, chief=None, targets=None):
+    """tolerance_wavefront's result from the sums (V, H, W, 10), the
+    wavelengths `wl` (W,) in lens units, the bundles' ray counts N (H, W),
+    the spectral `weights` (W,), `chief` (V, H, W) bool (None: all true) and
+    `targets` (broadcast to (H,), waves rms tilt removed).  An item whose
+    chief ray is lost has NaN for every value; rms and rms_tilt are NaN
+    where no ray entered"""
+    sums = np.array(sums, np.float64)
+    V, H, W, _ = sums.shape
+    chief = np.ones((V, H, W), bool) if chief is None else np.asarray(chief, bool)
+    sums[~chief] = np.nan
+    wl = np.asarray(wl, np.float64).reshape(W)
+    n = sums[..., 0]
+    with np.errstate(all="ignore"):
+        dbar = sums[..., 1]/n                                  # gauss_newton_wavefront's rms
+        rms = np.sqrt(np.maximum((sums[..., 2]/n - dbar*dbar)/(wl*wl), 0.))
+        rms = np.where(np.isnan(dbar), np.nan, rms)
+        ssr, _, nl = _tilt_fit(sums)
+        # the fit never raises the rms; rounding may, by an ulp, where the tilt is 0
+        rms_tilt = np.minimum((np.sqrt(ssr/nl)/wl).astype(np.float64), rms)
+        strehl = np.exp(-(2*np.pi*rms_tilt)**2)
+        transmitted = n/np.asarray(N, np.float64).reshape(H, W)
+        w = np.asarray(weights, np.float64).reshape(W)
+        poly_rms = np.sqrt((rms*rms*w).sum(-1)/w.sum())
+        poly_rms_tilt = np.sqrt((rms_tilt*rms_tilt*w).sum(-1)/w.sum())
+    out = dict(rms=rms, rms_tilt=rms_tilt, strehl=strehl, transmitted=transmitted,
+               chief=chief, poly_rms=poly_rms, poly_rms_tilt=poly_rms_tilt, sums=sums)
+    if targets is not None:
+        t = _wfe_targets(targets, H)
+        with np.errstate(invalid="ignore"):
+            out["passed"] = (poly_rms_tilt <= t).all(-1)
+        out["yield"] = float(out["passed"].mean())
+    return out
+
+
+def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), wavelengths=None,
+                        nrays=1000, distribution="hexapolar", compensate=None,
+                        spectral_weights=None, targets=None, engine=None, exact=False, chunk=None):
+    """The rms wavefront error of every perturbed lens at every field height
+    and wavelength, on the device: the wavefront counterpart of
+    ``tolerance`` and ``tolerance_mtf``.
+
+    `params` [(j, kind)] and `deltas` (V, P) are ``perturbed_tables``'; a
+    shape or tilt of the image surface is refused (it changes only the
+    reference sphere), its distance (a defocus) is not.  Each (height,
+    wavelength) bundle is aimed once for the NOMINAL lens and marched through
+    all V variants with clipping (no re-aiming).  Each variant has its own
+    reference sphere: opd()'s default radius of the nominal lens, centred on
+    the variant's chief-ray image point and turned by its last lens
+    surface's tilt.  Per chunk of variants there are three launches: the
+    chief rays to the image (rtx_trace_reduce_many), the chief rays' path
+    and sphere point (rtx_trace_opd_many), then every ray's residuals about
+    them, opd()'s chief-referenced t and py, reduced to the sums of a fit of
+    piston and tilt (rtx_trace_opd_many).  ``compensate="focus"`` refocuses
+    each variant first, as ``tolerance`` does.  `targets` (broadcast to (H,))
+    are the largest accepted polychromatic rms_tilt in waves.  `chunk`:
+    variants per launch (default: as many as fit in 1 GiB of tables and
+    tile rows); the results do not depend on it.  FP64 only.
+
+    Returns a dict: rms (V, H, W) the piston-removed rms in waves (lambda =
+    l/system.scale), rms_tilt (V, H, W) the residual rms after the
+    least-squares fit of 1, x, y (tilt removed), strehl = exp(-(2 pi
+    rms_tilt)^2) (Marechal), transmitted (V, H, W) the fraction of the rays
+    that enter, chief (V, H, W) true where the variant's chief ray reaches
+    the image (elsewhere every value is NaN), poly_rms and poly_rms_tilt
+    (V, H) the `spectral_weights` mean of rms^2 over the wavelengths,
+    square-rooted, sums (V, H, W, 10) rtx_trace_opd_many's, focus (V,) when
+    compensated, heights, wavelengths, params, deltas; with `targets` also
+    passed (V,) (every height within its target, NaN failing) and yield,
+    the fraction of variants that pass.  Every argument is checked before
+    any device work."""
+    from .engine import WFE_NSUMS
+    from .lazy import opd_spec
+    from .mtf import _spectral
+    from .surface_table import pack_system
+    if compensate not in (None, "focus"):
+        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    heights = list(heights)
+    H, W = len(heights), len(wavelengths)
+    sw = _spectral(spectral_weights, W)
+    if targets is not None:
+        targets = _wfe_targets(targets, H)
+    if chunk is not None and int(chunk) < 1:
+        raise ValueError("chunk must be >= 1")
+    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
+    nominal = np.stack([t for t, _, _ in packs])
+    rot0 = packs[0][2]
+    S = nominal.shape[1]
+    params = list(params)
+    deltas = np.asarray(deltas, np.float64)
+    if deltas.ndim == 1:
+        deltas = deltas[None]
+    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
+    for j, kind in params:
+        if j == S and kind != "distance":
+            raise ValueError("%s of the image surface %d changes only the reference sphere"
+                             % (kind, j))
+    V = deltas.shape[0]
+    eng = engine or default_engine()
+    fsys = copy.deepcopy(system) if compensate == "focus" else None
+    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
+    after, image = S - 1, S                                    # System indices
+    ei = system[image]
+    Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else np.eye(3)
+    origin0 = np.asarray(system[0].offset, np.float64)
+    nb = H*W
+    base = [opd_spec(system, system.track, system.origins, after, image,
+                     system.refractive_index(wavelengths[b % W], 0), float(nominal[b % W, S - 2]["n"]),
+                     np.reshape(y0, 3), np.reshape(u0, 3), np.zeros(3))
+            for b, (y0, u0) in enumerate(chiefs)]
+    wl = np.array([l/system.scale for l in wavelengths])
+    focus = None
+    sums = np.empty((V, H, W, WFE_NSUMS))
+    chief = np.empty((V, H, W), bool)
+    cdev = []
+    try:
+        for y0, u0 in chiefs:
+            cdev.append((eng.to_device(np.reshape(y0, (1, 3))), eng.to_device(np.reshape(u0, (1, 3))),
+                         None))
+        dev = [(y, u, None) for y, u in bundles]
+        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
+        step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 160, 3*nb)
+        if compensate == "focus":
+            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
+        for v0 in range(0, V, step):
+            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+            n = len(t)
+            if focus is not None:                              # system[-1].distance += shift
+                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
+                                                          focus[v0:v0 + n, None])
+            v, b = (a.reshape(-1) for a in np.meshgrid(np.arange(n), np.arange(nb), indexing="ij"))
+            items = np.stack([v*W + b % W, b], -1)
+            # 1. each variant's chief-ray image point
+            m = eng.trace_reduce_many(t.reshape(n*W, S), cdev, items, clip=True, rot0=rot0,
+                                      exact=exact).reshape(n, nb, 20)
+            ok = m[..., 4] == 1
+            xy = np.where(ok[..., None], m[..., 1:3], 0.)
+            # 2. its reference sphere
+            specs = np.empty((n, nb), wavefront_specs(base[0], t[:1, 0], xy[:1, 0], Ri, origin0,
+                                                      nominal[0, S - 1]).dtype)
+            for bi in range(nb):
+                w = bi % W
+                specs[:, bi] = wavefront_specs(base[bi], t[:, w], xy[:, bi], Ri, origin0,
+                                               nominal[w, S - 1])
+            specs = specs.reshape(-1)
+            march = t[:, :, :-1].reshape(n*W, S - 1)
+            # 3. the chief ray's path and sphere point, exactly (single-term sums)
+            c = eng.trace_opd_many(march, cdev, items, specs, clip=True, rot0=rot0,
+                                   exact=exact).reshape(n, nb, WFE_NSUMS)
+            ok &= c[..., 0] == 1
+            a0 = np.where(ok, c[..., 1], 0.).reshape(-1)
+            cen = np.where(ok[..., None], c[..., 3:5], 0.).reshape(-1, 2)
+            # 4. every ray's residuals about the chief ray's
+            s = eng.trace_opd_many(march, dev, items, specs, a0, cen, clip=True, rot0=rot0,
+                                   exact=exact)
+            sums[v0:v0 + n] = s.reshape(n, H, W, WFE_NSUMS)
+            chief[v0:v0 + n] = ok.reshape(n, H, W)
+    finally:
+        for y, u in bundles:
+            y.free(), u.free()
+        for y, u, _ in cdev:
+            y.free(), u.free()
+    Nb = np.array([y.shape[0] for y, _ in bundles], np.float64).reshape(H, W)
+    out = wavefront_tolerance_result(sums, wl, Nb, sw, chief, targets)
+    out.update(heights=np.asarray(heights, np.float64),
+               wavelengths=np.asarray(wavelengths, np.float64), params=params, deltas=deltas)
+    if focus is not None:
+        out["focus"] = focus
+    return out
