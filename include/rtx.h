@@ -885,6 +885,82 @@ int rtx_trace_opd_many(rtx_ctx *ctx, int nt, const rtx_surface *tables, int S,
                        const double *a0, const double *centers, int clip,
                        double *sums, unsigned flags);
 
+/* ---- Zernike decomposition of the wavefront ------------------------------ */
+/*
+ * rtx_trace_opd_many's items and per-ray residuals, reduced to the sums of
+ * a least-squares fit of the Zernike polynomials Z_1 .. Z_J to a.
+ * Arguments as rtx_trace_opd_many, plus the radial order `order` (0 ..
+ * RTX_ZRN_MAX_ORDER; J = (order+1)(order+2)/2 <= 45) and rho (host, nitems
+ * doubles), item i's normalisation radius: the pupil point of a ray is
+ * (u, v) = (x, y)/rho.  Per ray a, x, y and the entry rule (a, x and y all
+ * finite) are rtx_trace_opd_many's, bit for bit.
+ *
+ * Basis: Noll's order, orthonormal on the unit disc (mean of Z_j Z_k over
+ * the disc = delta_jk).  Z_j has radial order n and azimuthal order m,
+ *   Z = sqrt(n+1) R_n^0(r)                  m = 0
+ *   Z = sqrt(2(n+1)) R_n^m(r) cos(m theta)  j even
+ *   Z = sqrt(2(n+1)) R_n^m(r) sin(m theta)  j odd
+ * with theta from the image-frame x axis (so Z2 = 2u, Z3 = 2v, Z4 =
+ * sqrt3 (2r^2 - 1), Z5 = sqrt6 r^2 sin 2theta, Z6 = sqrt6 r^2 cos 2theta,
+ * Z7 = sqrt8 (3r^3 - 2r) sin theta, Z11 = sqrt5 (6r^4 - 6r^2 + 1)).  The
+ * device evaluates it without atan2, every operation separately rounded:
+ * u = x/rho, v = y/rho, s = u^2 + v^2, R_n^m/r^m by Horner in s with its
+ * integer coefficients c_k, (u + iv)^m by repeated complex multiplication,
+ * Z = (N Q) Re or Im of it with N the rounded sqrt.
+ *
+ * sums: host (nitems, E), E = (J+1)(J+2)/2: the upper triangle, row-major,
+ * of the Gram sums of v = (a, Z_1, .., Z_J) over the rays that enter:
+ *   sum a^2, sum a Z_1 .. sum a Z_J, sum Z_1 Z_1, sum Z_1 Z_2, .. sum Z_J Z_J
+ * so sum a Z_1 = sum a and sum Z_1 Z_1 = n exactly (Z_1 = 1).  r2max: host
+ * (nitems,), the largest x^2 + y^2 (each rounded) over the rays that enter,
+ * 0 for none; exact.  Zeros for N = 0.
+ *
+ * Deterministic: each 512-ray tile's row (each entry added over the tile's
+ * rays in ray order by one thread, every product and sum rounded once; the
+ * max is exact) goes to the tile's own row, and a second kernel adds each
+ * item's rows in tile order (no atomics).  An item's bits depend only on
+ * its rays, table, spec, a0, centre and rho.
+ *
+ * Error bound, eps = 2^-52, in two parts:
+ *  (a) one basis value against the exact Z_j at the same (x, y)/rho, at
+ *      the normalised radius r = |(x, y)|/rho and R = max(1, r):
+ *        |Z~_j - Z_j| <= (n+2)^2 eps N_j A_j R^n
+ *      N_j = sqrt(n+1) or sqrt(2(n+1)), A_j = sum_k |c_k| the sum of R_n^m's
+ *      coefficient magnitudes (R_8^0: 321).  Derivation, u = eps/2:
+ *      rounding u, v perturbs the point by <= u r, worth n^2 u sup|Z| over
+ *      the disc of radius R by Kellogg's bound |grad p| <= n^2 sup|p| / R,
+ *      and sup|Z| <= N A R^n; s carries 2u, worth 2K u N A R^n through
+ *      |dQ/ds| <= K A R^(2K-2); Horner of degree K adds 2K u N A R^n; each
+ *      complex product adds sqrt2 * 2u |C||w|, so C_m is within 2 sqrt2 m
+ *      u R^m; N and the two products add 3u.  The sum, n^2 + 4K + 2.9m + 3
+ *      <= (n+2)^2 - 1 with n = 2K + m, times u, is within the bound.
+ *  (b) the summation of the rounded products of the device values:
+ *        |sum - sum of the products| <= (512 + ceil(N/512)) eps sum|term|
+ *      (a tile's depth is 511 additions and the product's rounding, each
+ *      u, and ceil(N/512) - 1 additions join the tiles).
+ * A sum's error against the exact sums of the exact basis is therefore
+ * within (b) plus sum over the rays of E_p |v_q| + |v_p| E_q + E_p E_q with
+ * E the bound (a) of each factor (0 for a).  Counts and r2max are exact.
+ *
+ * FP64 only, fast or RTX_EXACT: RTX_F32 returns RTX_E_UNSUPPORTED.
+ * RTX_E_BADARG, before any device work or allocation: every refusal of
+ * rtx_trace_opd_many; a NULL rho or r2max; an order outside 0 ..
+ * RTX_ZRN_MAX_ORDER; a non-finite or non-positive rho.  The tile rows
+ * (E + 1 doubles per tile) are kept in the context with the tables, items
+ * and specs: RTX_E_NOMEM before allocating when they do not fit.
+ * Synchronous; rtx_last_kernel_ms covers the two kernels.
+ */
+#define RTX_ZRN_MAX_ORDER 8
+int rtx_trace_zernike_many(rtx_ctx *ctx, int nt, const rtx_surface *tables,
+                           int S, const double *rot0, int dtype, int nb,
+                           const int64_t *N, const void *const *y0,
+                           const void *const *u0, int64_t nitems,
+                           const int32_t *item_table,
+                           const int32_t *item_bundle, const rtx_opd *specs,
+                           const double *a0, const double *centers, int clip,
+                           int order, const double *rho, double *sums,
+                           double *r2max, unsigned flags);
+
 /* ---- launch rays generated in HBM (SURVEY 8f-2) -------------------------- */
 /*
  * The pupil grids of pupil_distribution (rayopt/utils.py:118-199), Pupil.map

@@ -20,6 +20,7 @@ from .psf import psfs  # noqa: F401
 from .tolerance import (tolerance, tolerance_mtf, tolerance_wavefront,  # noqa: F401
                         perturbed_tables, sensitivity_deltas, monte_carlo_deltas,
                         record_tangents)
+from .zernike import tolerance_zernike, zernike  # noqa: F401
 from .optimize import (spot_jacobian, optimize_spot, wavefront_jacobian,  # noqa: F401
                        optimize_wavefront, mtf_jacobian, optimize_mtf)
 

@@ -65,6 +65,8 @@ SYMBOLS = {
                                    _vp, _i, _vp, _u]),
     "rtx_trace_opd_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
                                 _vp, _vp, _vp, _i, _vp, _u]),
+    "rtx_trace_zernike_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
+                                    _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_otf_many": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp,
                                 _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _u]),
     "rtx_trace_opd": (_i, [_vp, _vp, _i, _vp, _i, _i64, _vp, _vp, _i, _vp, _vp, _vp, _u]),

@@ -1618,9 +1618,11 @@ template <typename T, int MODE>
 int launch_epi_kernel(rtx_ctx* ctx, unsigned flags, long long tiles, const EpiParams<T>& p) {
     constexpr int RPT = 2, threads = 256;
     static_assert(threads * RPT == EPI_TILE, "epi_kernel's tile");
-    // the table, its barrier and (EPI_OTF) the tile's staged rays
+    // the table, its barrier and (EPI_OTF, EPI_ZRN) the tile's staged rays
     size_t smem = (((size_t)p.S * sizeof(DevSurf<T>) + 127) & ~size_t(127)) +
-                  (MODE == EPI_OTF ? 128 + 4 * EPI_TILE * sizeof(double) : 16);
+                  (MODE == EPI_OTF   ? 128 + 4 * EPI_TILE * sizeof(double)
+                   : MODE == EPI_ZRN ? 128 + zrn_smem_doubles(p.zrn_order) * sizeof(double)
+                                     : 16);
     if ((int)smem > ctx->max_smem_optin) return RTX_E_UNSUPPORTED;
     auto go = [&](auto kern) -> int {
         if (smem > 48 * 1024)
@@ -1712,11 +1714,12 @@ int rtx_trace_reduce(rtx_ctx* ctx, const rtx_surface* surf, int S, const double*
 namespace {
 // rtx_trace_reduce_many (MODE EPI_MANY, W = RTX_NMOMENTS, centres of 4
 // doubles), rtx_trace_otf_many (EPI_OTF, W its row width, centres of 2) and
-// rtx_trace_opd_many (EPI_WFE, W = RTX_NMOMENTS, no centres): the launch-wide
+// rtx_trace_opd_many (EPI_WFE, W = RTX_NMOMENTS, no centres) and
+// rtx_trace_zernike_many (EPI_ZRN, W = zrn_row, no centres): the launch-wide
 // tile list, the epilogue kernel over it, then the second pass that adds
 // each item's W-wide tile rows in tile order into out (host, (nitems, W)).
 // `consts` go to the device after the items (EPI_OTF: z, nu; EPI_WFE: the
-// WfeItem of every item).
+// WfeItem of every item; EPI_ZRN: those, then every item's rho).
 template <typename T, int MODE>
 int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
                const int64_t* N, const void* const* y0, const void* const* u0, long long nitems,
@@ -1779,7 +1782,8 @@ int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const dou
     p.tiles = tiles;
     p.part = part;
     p.otf_zf = dconsts;
-    if constexpr (MODE == EPI_WFE) p.wfe = reinterpret_cast<const WfeItem*>(dconsts);
+    if constexpr (MODE == EPI_WFE || MODE == EPI_ZRN) p.wfe = reinterpret_cast<const WfeItem*>(dconsts);
+    if constexpr (MODE == EPI_ZRN) p.zrn_rho = dconsts + (size_t)nitems * WFE_ITEM_DOUBLES;
     rc = timed(ctx, [&]() -> int {
         if (tiles > 0) {
             int rc = launch_epi_kernel<T, MODE>(ctx, flags, tiles, p);
@@ -1789,8 +1793,9 @@ int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const dou
             many_sum_kernel<<<cap_grid(ctx, (nitems * RTX_NMOMENTS + 255) / 256, 8), 256, 0,
                               ctx->stream>>>(ditems, nitems, part, dm);
         else
-            many_rows_kernel<<<cap_grid(ctx, (nitems * W + 255) / 256, 8), 256, 0, ctx->stream>>>(
-                ditems, nitems, W, part, dm);
+            many_rows_kernel<MODE == EPI_ZRN>
+                <<<cap_grid(ctx, (nitems * W + 255) / 256, 8), 256, 0, ctx->stream>>>(
+                    ditems, nitems, W, part, dm);
         ctx->launches++;
         return (int)cudaGetLastError();
     });
@@ -1800,8 +1805,8 @@ int trace_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const dou
     return 0;
 }
 
-// the refusals rtx_trace_reduce_many, rtx_trace_otf_many and
-// rtx_trace_opd_many share
+// the refusals rtx_trace_reduce_many, rtx_trace_otf_many,
+// rtx_trace_opd_many and rtx_trace_zernike_many share
 int check_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, int nb, const int64_t* N,
                const void* const* y0, const void* const* u0, int64_t nitems,
                const int32_t* item_table, const int32_t* item_bundle) {
@@ -1882,17 +1887,14 @@ int rtx_trace_otf_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, c
     });
 }
 
-int rtx_trace_opd_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
-                       int dtype, int nb, const int64_t* N, const void* const* y0,
-                       const void* const* u0, int64_t nitems, const int32_t* item_table,
-                       const int32_t* item_bundle, const rtx_opd* specs, const double* a0,
-                       const double* centers, int clip, double* sums, unsigned flags) {
-    static_assert(RTX_WFE_NSUMS == WFE_NSUMS && WFE_NSUMS <= RTX_NMOMENTS, "rtx_trace_opd_many's row");
-    if (!sums || !specs) return RTX_E_BADARG;
-    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
-    if (rc) return rc;
-    // every item's WfeItem, checked before any device work
-    std::vector<double> consts((size_t)nitems * WFE_ITEM_DOUBLES);
+}  // extern "C"
+
+namespace {
+// every item's WfeItem (rtx_trace_opd_many's and rtx_trace_zernike_many's
+// device constants) into consts, checked before any device work
+int wfe_items(long long nitems, const rtx_opd* specs, const double* a0, const double* centers,
+              std::vector<double>& consts) {
+    consts.assign((size_t)nitems * WFE_ITEM_DOUBLES, 0.0);
     for (long long i = 0; i < nitems; ++i) {
         const rtx_opd& o = specs[i];
         WfeItem w;
@@ -1915,6 +1917,24 @@ int rtx_trace_opd_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, c
         if (w.radius == 0.0) return RTX_E_BADARG;
         memcpy(consts.data() + (size_t)i * WFE_ITEM_DOUBLES, &w, sizeof(w));
     }
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int rtx_trace_opd_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, const double* rot0,
+                       int dtype, int nb, const int64_t* N, const void* const* y0,
+                       const void* const* u0, int64_t nitems, const int32_t* item_table,
+                       const int32_t* item_bundle, const rtx_opd* specs, const double* a0,
+                       const double* centers, int clip, double* sums, unsigned flags) {
+    static_assert(RTX_WFE_NSUMS == WFE_NSUMS && WFE_NSUMS <= RTX_NMOMENTS, "rtx_trace_opd_many's row");
+    if (!sums || !specs) return RTX_E_BADARG;
+    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
+    if (rc) return rc;
+    std::vector<double> consts;
+    rc = wfe_items(nitems, specs, a0, centers, consts);
+    if (rc) return rc;
     return dispatch(dtype, [&](auto t) -> int {
         using T = decltype(t);
         if constexpr (sizeof(T) != 8) {
@@ -1930,6 +1950,48 @@ int rtx_trace_opd_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S, c
             for (long long i = 0; i < nitems; ++i)
                 memcpy(sums + (size_t)i * RTX_WFE_NSUMS, rows.data() + (size_t)i * RTX_NMOMENTS,
                        RTX_WFE_NSUMS * sizeof(double));
+            return 0;
+        }
+    });
+}
+
+int rtx_trace_zernike_many(rtx_ctx* ctx, int nt, const rtx_surface* tables, int S,
+                           const double* rot0, int dtype, int nb, const int64_t* N,
+                           const void* const* y0, const void* const* u0, int64_t nitems,
+                           const int32_t* item_table, const int32_t* item_bundle,
+                           const rtx_opd* specs, const double* a0, const double* centers, int clip,
+                           int order, const double* rho, double* sums, double* r2max,
+                           unsigned flags) {
+    static_assert(RTX_ZRN_MAX_ORDER == ZRN_MAX_ORDER, "rtx_trace_zernike_many's orders");
+    if (!sums || !specs || !rho || !r2max) return RTX_E_BADARG;
+    int rc = check_many(ctx, nt, tables, S, nb, N, y0, u0, nitems, item_table, item_bundle);
+    if (rc) return rc;
+    if (order < 0 || order > RTX_ZRN_MAX_ORDER) return RTX_E_BADARG;
+    std::vector<double> consts;
+    rc = wfe_items(nitems, specs, a0, centers, consts);
+    if (rc) return rc;
+    for (long long i = 0; i < nitems; ++i)
+        if (!(std::isfinite(rho[i]) && rho[i] > 0.0)) return RTX_E_BADARG;
+    consts.insert(consts.end(), rho, rho + nitems);
+    return dispatch(dtype, [&](auto t) -> int {
+        using T = decltype(t);
+        if constexpr (sizeof(T) != 8) {
+            return RTX_E_UNSUPPORTED;  // as rtx_trace_opd_many
+        } else {
+            EpiParams<T> p;
+            memset(&p, 0, sizeof(p));
+            p.zrn_order = order;
+            const int W = zrn_row(order), E = W - 1;
+            std::vector<double> rows((size_t)nitems * W);
+            int rc = trace_many<T, EPI_ZRN>(ctx, nt, tables, S, rot0, N, y0, u0, nitems, item_table,
+                                            item_bundle, nullptr, 2, clip, W, consts, rows.data(),
+                                            flags, p);
+            if (rc) return rc;
+            for (long long i = 0; i < nitems; ++i) {
+                const double* r = rows.data() + (size_t)i * W;
+                memcpy(sums + (size_t)i * E, r, (size_t)E * sizeof(double));
+                r2max[i] = r[E];
+            }
             return 0;
         }
     });

@@ -54,6 +54,7 @@ def spot_spec(z, bins, range, center, radial=False, offsets=None):
 # mirrors `struct rtx_otf` (include/rtx.h)
 OTF_MAX_PLANES, OTF_MAX_FREQS = 16, 256
 WFE_NSUMS = 10      # RTX_WFE_NSUMS: n, sum a, a^2, x, y, x^2, xy, y^2, ax, ay
+ZRN_MAX_ORDER = 8   # RTX_ZRN_MAX_ORDER
 OTF_SLOT, OTF_BLOCK = 16384, 16      # RTX_OTF_SLOT, RTX_OTF_BLOCK
 MAX_PARAMS, JAC_SLOT = 64, 16384     # RTX_MAX_PARAMS, RTX_JAC_SLOT
 OTF_DTYPE = np.dtype([("planes", "<i4"), ("nfreq", "<i4"), ("dnu", "<f8"), ("c", "<f8", (2,)),
@@ -698,8 +699,8 @@ class Engine:
 
     @staticmethod
     def _many_args(tables, bundles, items):
-        """the checked arguments trace_reduce_many, trace_otf_many and
-        trace_opd_many share:
+        """the checked arguments trace_reduce_many, trace_otf_many,
+        trace_opd_many and trace_zernike_many share:
         (tables, dtype, items, N, y0s, u0s, item tables, item bundles)"""
         tables = np.ascontiguousarray(tables, SURFACE_DTYPE)
         if tables.ndim != 2 or tables.shape[0] < 1 or tables.shape[1] < 1:
@@ -773,6 +774,21 @@ class Engine:
             K, ptr(z), F, ptr(nu), ptr(sums), ptr(count), self._flags(exact, False)))
         return sums[..., 0] + 1j*sums[..., 1], count
 
+    @staticmethod
+    def _wfe_args(n, specs, a0, centers):
+        """the checked per-item arguments trace_opd_many and
+        trace_zernike_many share: (spec records, a0, centres)"""
+        if isinstance(specs, np.ndarray) and specs.dtype == OPD_DTYPE:
+            rec = np.ascontiguousarray(specs.reshape(-1))
+        else:
+            rec = np.concatenate([_opd_record(s) for s in specs]) if len(specs) else \
+                np.zeros(0, OPD_DTYPE)
+        if len(rec) != n:
+            raise ValueError("need one spec per item: %d specs for %d items" % (len(rec), n))
+        a = None if a0 is None else np.ascontiguousarray(a0, np.float64).reshape(n)
+        c = None if centers is None else np.ascontiguousarray(centers, np.float64).reshape(n, 2)
+        return rec, a, c
+
     def trace_opd_many(self, tables, bundles, items, specs, a0=None, centers=None, clip=False,
                        rot0=None, exact=False):
         """rtx_trace_opd_many: `tables` (nt, S) records of the march to
@@ -786,21 +802,36 @@ class Engine:
         depend on its own item only."""
         tables, dtype, items, N, y0s, u0s, it, ib = self._many_args(tables, bundles, items)
         n = len(items)
-        if isinstance(specs, np.ndarray) and specs.dtype == OPD_DTYPE:
-            rec = np.ascontiguousarray(specs.reshape(-1))
-        else:
-            rec = np.concatenate([_opd_record(s) for s in specs]) if len(specs) else \
-                np.zeros(0, OPD_DTYPE)
-        if len(rec) != n:
-            raise ValueError("need one spec per item: %d specs for %d items" % (len(rec), n))
-        a = None if a0 is None else np.ascontiguousarray(a0, np.float64).reshape(n)
-        c = None if centers is None else np.ascontiguousarray(centers, np.float64).reshape(n, 2)
+        rec, a, c = self._wfe_args(n, specs, a0, centers)
         sums = np.zeros((n, WFE_NSUMS))
         check(self.lib.rtx_trace_opd_many(
             self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
             len(bundles), ptr(N), y0s, u0s, n, ptr(it), ptr(ib), ptr(rec), ptr(a), ptr(c),
             int(bool(clip)), ptr(sums), self._flags(exact, False)))
         return sums
+
+    def trace_zernike_many(self, tables, bundles, items, specs, rho, order, a0=None,
+                           centers=None, clip=False, rot0=None, exact=False):
+        """rtx_trace_zernike_many: trace_opd_many's arguments, the radial
+        `order` (0..8) and `rho` (nitems,) each item's normalisation radius.
+        Returns (sums (nitems, E), r2max (nitems,)): E = (J+1)(J+2)/2, J =
+        (order+1)(order+2)/2, the upper triangle row-major of the Gram sums
+        of (a, Z_1 .. Z_J) at (x, y)/rho (Noll's orthonormal Zernikes) over
+        the rays whose a, x, y are finite, and the largest x^2 + y^2 of those
+        rays; from one launch; FP64 only; each row's bits depend on its own
+        item only."""
+        tables, dtype, items, N, y0s, u0s, it, ib = self._many_args(tables, bundles, items)
+        n = len(items)
+        rec, a, c = self._wfe_args(n, specs, a0, centers)
+        r = np.ascontiguousarray(rho, np.float64).reshape(n)
+        J = (int(order) + 1)*(int(order) + 2)//2
+        sums = np.zeros((n, (J + 1)*(J + 2)//2))
+        r2max = np.zeros(n)
+        check(self.lib.rtx_trace_zernike_many(
+            self.ctx, len(tables), ptr(tables), tables.shape[1], ptr(_rot0(rot0)), _code(dtype),
+            len(bundles), ptr(N), y0s, u0s, n, ptr(it), ptr(ib), ptr(rec), ptr(a), ptr(c),
+            int(bool(clip)), int(order), ptr(r), ptr(sums), ptr(r2max), self._flags(exact, False)))
+        return sums, r2max
 
     @staticmethod
     def rms_finite_from_moments(m):

@@ -644,6 +644,76 @@ def wavefront_tolerance_result(sums, wl, N, weights, chief=None, targets=None):
     return out
 
 
+class _WavefrontRef:
+    """The chief-ray reference of the rms wavefront, shared by
+    tolerance_wavefront and tolerance_zernike: each (height, wavelength)
+    bundle's nominal opd() spec (`base`), the image surface's rot_normal
+    `Ri` and the object's offset `origin0`; `chief` makes the per-chunk
+    launches that refer every variant's rays to its own chief ray"""
+
+    def __init__(self, system, nominal, wavelengths, chiefs):
+        from .lazy import opd_spec
+        W, S = len(wavelengths), nominal.shape[1]
+        after, image = S - 1, S                                # System indices
+        ei = system[image]
+        self.Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else np.eye(3)
+        self.origin0 = np.asarray(system[0].offset, np.float64)
+        self.base = [opd_spec(system, system.track, system.origins, after, image,
+                              system.refractive_index(wavelengths[b % W], 0),
+                              float(nominal[b % W, S - 2]["n"]), np.reshape(y0, 3),
+                              np.reshape(u0, 3), np.zeros(3))
+                     for b, (y0, u0) in enumerate(chiefs)]
+        self.nominal, self.chiefs, self.W = nominal, chiefs, W
+        self.cdev = []
+
+    def upload(self, eng):
+        """the chief rays as 1-ray device bundles (freed by `free`)"""
+        for y0, u0 in self.chiefs:
+            self.cdev.append((eng.to_device(np.reshape(y0, (1, 3))),
+                              eng.to_device(np.reshape(u0, (1, 3))), None))
+        return self.cdev
+
+    def free(self):
+        for y, u, _ in self.cdev:
+            y.free(), u.free()
+        self.cdev = []
+
+    def chief(self, eng, t, rot0, exact):
+        """For the variants' full tables t (n, W, S): (march (n*W, S-1),
+        items (n*nb, 2) variant-major, specs (n*nb,), a0 (n*nb,), centres
+        (n*nb, 2), ok (n, nb)) -- the march tables and the per-item
+        arguments of rtx_trace_opd_many or rtx_trace_zernike_many whose
+        residuals are opd()'s chief-referenced t and py; ok is false where
+        the chief ray is lost (a0 and the centre are 0 there)"""
+        from .engine import WFE_NSUMS
+        n, W, S = t.shape
+        nb = len(self.chiefs)
+        nominal, base, Ri, origin0, cdev = self.nominal, self.base, self.Ri, self.origin0, self.cdev
+        v, b = (a.reshape(-1) for a in np.meshgrid(np.arange(n), np.arange(nb), indexing="ij"))
+        items = np.stack([v*W + b % W, b], -1)
+        # 1. each variant's chief-ray image point
+        m = eng.trace_reduce_many(t.reshape(n*W, S), cdev, items, clip=True, rot0=rot0,
+                                  exact=exact).reshape(n, nb, 20)
+        ok = m[..., 4] == 1
+        xy = np.where(ok[..., None], m[..., 1:3], 0.)
+        # 2. its reference sphere
+        specs = np.empty((n, nb), wavefront_specs(base[0], t[:1, 0], xy[:1, 0], Ri, origin0,
+                                                  nominal[0, S - 1]).dtype)
+        for bi in range(nb):
+            w = bi % W
+            specs[:, bi] = wavefront_specs(base[bi], t[:, w], xy[:, bi], Ri, origin0,
+                                           nominal[w, S - 1])
+        specs = specs.reshape(-1)
+        march = t[:, :, :-1].reshape(n*W, S - 1)
+        # 3. the chief ray's path and sphere point, exactly (single-term sums)
+        c = eng.trace_opd_many(march, cdev, items, specs, clip=True, rot0=rot0,
+                               exact=exact).reshape(n, nb, WFE_NSUMS)
+        ok &= c[..., 0] == 1
+        a0 = np.where(ok, c[..., 1], 0.).reshape(-1)
+        cen = np.where(ok[..., None], c[..., 3:5], 0.).reshape(-1, 2)
+        return march, items, specs, a0, cen, ok
+
+
 def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), wavelengths=None,
                         nrays=1000, distribution="hexapolar", compensate=None,
                         spectral_weights=None, targets=None, engine=None, exact=False, chunk=None):
@@ -681,7 +751,6 @@ def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), waveleng
     the fraction of variants that pass.  Every argument is checked before
     any device work."""
     from .engine import WFE_NSUMS
-    from .lazy import opd_spec
     from .mtf import _spectral
     from .surface_table import pack_system
     if compensate not in (None, "focus"):
@@ -711,24 +780,14 @@ def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), waveleng
     eng = engine or default_engine()
     fsys = copy.deepcopy(system) if compensate == "focus" else None
     bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    after, image = S - 1, S                                    # System indices
-    ei = system[image]
-    Ri = np.asarray(ei.rot_normal, float) if getattr(ei, "rotated", False) else np.eye(3)
-    origin0 = np.asarray(system[0].offset, np.float64)
+    ref = _WavefrontRef(system, nominal, wavelengths, chiefs)
     nb = H*W
-    base = [opd_spec(system, system.track, system.origins, after, image,
-                     system.refractive_index(wavelengths[b % W], 0), float(nominal[b % W, S - 2]["n"]),
-                     np.reshape(y0, 3), np.reshape(u0, 3), np.zeros(3))
-            for b, (y0, u0) in enumerate(chiefs)]
     wl = np.array([l/system.scale for l in wavelengths])
     focus = None
     sums = np.empty((V, H, W, WFE_NSUMS))
     chief = np.empty((V, H, W), bool)
-    cdev = []
     try:
-        for y0, u0 in chiefs:
-            cdev.append((eng.to_device(np.reshape(y0, (1, 3))), eng.to_device(np.reshape(u0, (1, 3))),
-                         None))
+        cdev = ref.upload(eng)
         dev = [(y, u, None) for y, u in bundles]
         tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
         step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 160, 3*nb)
@@ -740,28 +799,7 @@ def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), waveleng
             if focus is not None:                              # system[-1].distance += shift
                 t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
                                                           focus[v0:v0 + n, None])
-            v, b = (a.reshape(-1) for a in np.meshgrid(np.arange(n), np.arange(nb), indexing="ij"))
-            items = np.stack([v*W + b % W, b], -1)
-            # 1. each variant's chief-ray image point
-            m = eng.trace_reduce_many(t.reshape(n*W, S), cdev, items, clip=True, rot0=rot0,
-                                      exact=exact).reshape(n, nb, 20)
-            ok = m[..., 4] == 1
-            xy = np.where(ok[..., None], m[..., 1:3], 0.)
-            # 2. its reference sphere
-            specs = np.empty((n, nb), wavefront_specs(base[0], t[:1, 0], xy[:1, 0], Ri, origin0,
-                                                      nominal[0, S - 1]).dtype)
-            for bi in range(nb):
-                w = bi % W
-                specs[:, bi] = wavefront_specs(base[bi], t[:, w], xy[:, bi], Ri, origin0,
-                                               nominal[w, S - 1])
-            specs = specs.reshape(-1)
-            march = t[:, :, :-1].reshape(n*W, S - 1)
-            # 3. the chief ray's path and sphere point, exactly (single-term sums)
-            c = eng.trace_opd_many(march, cdev, items, specs, clip=True, rot0=rot0,
-                                   exact=exact).reshape(n, nb, WFE_NSUMS)
-            ok &= c[..., 0] == 1
-            a0 = np.where(ok, c[..., 1], 0.).reshape(-1)
-            cen = np.where(ok[..., None], c[..., 3:5], 0.).reshape(-1, 2)
+            march, items, specs, a0, cen, ok = ref.chief(eng, t, rot0, exact)
             # 4. every ray's residuals about the chief ray's
             s = eng.trace_opd_many(march, dev, items, specs, a0, cen, clip=True, rot0=rot0,
                                    exact=exact)
@@ -770,8 +808,7 @@ def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), waveleng
     finally:
         for y, u in bundles:
             y.free(), u.free()
-        for y, u, _ in cdev:
-            y.free(), u.free()
+        ref.free()
     Nb = np.array([y.shape[0] for y, _ in bundles], np.float64).reshape(H, W)
     out = wavefront_tolerance_result(sums, wl, Nb, sw, chief, targets)
     out.update(heights=np.asarray(heights, np.float64),
