@@ -51,15 +51,10 @@ from .engine import (Engine, default_engine, jacobian_sums_unpack, otf_jacobian_
                      wavefront_sums_unpack)
 from .lazy import opd_spec
 from .mtf import _check_freqs, _spectral, poly_otf
-from .surface_table import RTX_MAX_ASPH, SURFACE_DTYPE, pack_system
-from .tolerance import _chief, launch_bundles, perturbed_tables, record_tangents
+from .surface_table import RTX_MAX_ASPH, SURFACE_DTYPE
+from .tolerance import _centers, _nominal, launch_bundles, perturbed_tables, record_tangents
 
 OPT_KINDS = ("curvature", "conic", "distance") + tuple("asph%d" % i for i in range(RTX_MAX_ASPH))
-
-
-def _nominal(system, wavelengths):
-    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
-    return np.stack([t for t, _, _ in packs]), packs[0][2]
 
 
 class _Bundles:
@@ -74,8 +69,7 @@ class _Bundles:
         self.rays, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
         self.chiefs = chiefs
         try:
-            self.centers = np.array([_chief(eng, self.nominal[b % self.W], self.rot0, y, u, exact)
-                                     for b, (y, u) in enumerate(chiefs)])
+            self.centers = _centers(eng, self.nominal, self.rot0, chiefs, exact)
         except Exception:
             self.close()
             raise

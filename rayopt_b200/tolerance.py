@@ -19,7 +19,7 @@ import math
 import numpy as np
 
 from .engine import Engine, default_engine
-from .surface_table import F_ROTATED, RTX_MAX_ASPH, SURFACE_DTYPE
+from .surface_table import F_ROTATED, RTX_MAX_ASPH, SURFACE_DTYPE, pack_system
 
 KINDS = ("curvature", "conic", "distance", "tilt_x", "tilt_y", "index") + tuple(
     "asph%d" % i for i in range(RTX_MAX_ASPH))
@@ -239,14 +239,25 @@ def monte_carlo_deltas(tol, trials, seed=None):
     return np.random.default_rng(seed).uniform(-tol, tol, (int(trials), len(tol)))
 
 
-def _chief(eng, table, rot0, y0, u0, exact):
-    """(y_x, y_y, u_x, u_y) of one launch ray at the last surface of `table`,
-    zeros where it does not get there"""
-    Y, _, I, _ = eng.trace(table, y0, u0, clip=True, rot0=rot0, keep_last=True, exact=exact,
-                           want=("y", "i"))
-    with np.errstate(all="ignore"):
-        c = np.r_[Y[0, 0, :2], I[0, 0, :2]/I[0, 0, 2]].astype(np.float64)
-    return c if np.all(np.isfinite(c)) else np.zeros(4)
+def _nominal(system, wavelengths):
+    """the nominal lens's (W, S) tables, one per wavelength, and its rot0"""
+    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
+    return np.stack([t for t, _, _ in packs]), packs[0][2]
+
+
+def _centers(eng, nominal, rot0, chiefs, exact):
+    """(bundles, 4) (y_x, y_y, u_x, u_y) of each bundle's chief ray (the
+    launch rays `chiefs` of launch_bundles) at the last surface of
+    nominal[b % W], zeros where it does not get there"""
+    out = np.zeros((len(chiefs), 4))
+    for b, (y0, u0) in enumerate(chiefs):
+        Y, _, I, _ = eng.trace(nominal[b % len(nominal)], y0, u0, clip=True, rot0=rot0,
+                               keep_last=True, exact=exact, want=("y", "i"))
+        with np.errstate(all="ignore"):
+            c = np.r_[Y[0, 0, :2], I[0, 0, :2]/I[0, 0, 2]].astype(np.float64)
+        if np.all(np.isfinite(c)):
+            out[b] = c
+    return out
 
 
 def launch_bundles(system, heights, wavelengths, nrays, distribution, engine):
@@ -335,6 +346,116 @@ def _focus(eng, fsys, nominal, params, deltas, l, rot0, step, exact):
     return focus
 
 
+def check_fields(system, heights, wavelengths, compensate, chunk):
+    """(heights, wavelengths) as lists, after the refusals of the arguments
+    every tolerance analysis takes (ValueError)"""
+    if compensate not in (None, "focus"):
+        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
+    if chunk is not None and int(chunk) < 1:
+        raise ValueError("chunk must be >= 1, got %r" % (chunk,))
+    heights = list(heights)
+    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
+    if not heights or not wavelengths:
+        raise ValueError("need at least one height and one wavelength")
+    return heights, wavelengths
+
+
+class VariantMarch:
+    """The host side of every tolerance analysis, whose arguments it takes
+    (heights and wavelengths from check_fields).  On construction: the
+    nominal lens packed per wavelength (`nominal` (W, S), `rot0`),
+    perturbed_tables' refusals of `params` and `deltas` (V, P) and, for a
+    `wavefront` analysis, of a shape or tilt of the image surface (it
+    changes only the reference sphere), all before any device work; then
+    the launch bundles of the nominal lens (`dev`, height-major, `chiefs`
+    their chief rays, `counts` (H, W) their rays) and, for a `wavefront`
+    analysis, the chief-ray reference `ref` on the device.  Everything it
+    put on the device is freed when the ``with`` block it opens ends, or
+    when construction fails."""
+
+    def __init__(self, system, params, deltas, heights, wavelengths, nrays, distribution,
+                 compensate, chunk, engine, exact, wavefront=False):
+        self.nominal, self.rot0 = _nominal(system, wavelengths)
+        S = self.nominal.shape[1]
+        self.params = list(params)
+        deltas = np.asarray(deltas, np.float64)
+        self.deltas = deltas[None] if deltas.ndim == 1 else deltas
+        perturbed_tables(self.nominal, self.params, self.deltas[:0])
+        for j, kind in self.params:
+            if wavefront and j == S and kind != "distance":
+                raise ValueError("%s of the image surface %d changes only the reference sphere"
+                                 % (kind, j))
+        self.V, self.H, self.W = len(self.deltas), len(heights), len(wavelengths)
+        self.heights, self.wavelengths = heights, wavelengths
+        self.compensate, self.chunk, self.exact = compensate, chunk, exact
+        self.focus = None
+        self.eng = engine or default_engine()
+        # System.pupil's result depends on the calls made before it: the focus
+        # bundle is aimed on a copy taken before any
+        self.fsys = copy.deepcopy(system) if compensate == "focus" else None
+        self.bundles, self.chiefs = launch_bundles(system, heights, wavelengths, nrays,
+                                                   distribution, self.eng)
+        self.dev = [(y, u, None) for y, u in self.bundles]
+        self.counts = np.array([y.shape[0] for y, _ in self.bundles],
+                               np.float64).reshape(self.H, self.W)
+        self.ref = None
+        try:
+            if wavefront:
+                self.ref = _WavefrontRef(system, self.nominal, wavelengths, self.chiefs)
+                self.ref.upload(self.eng)
+        except BaseException:
+            self.close()
+            raise
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def close(self):
+        for y, u in self.bundles:
+            y.free(), u.free()
+        self.bundles = []
+        if self.ref is not None:
+            self.ref.free()
+
+    def chunks(self, row_bytes=160, items_per_variant=0):
+        """Refocus every variant when compensating, then yield (v0, t, items)
+        for each chunk of n variants v0 .. v0+n-1: t (n, W, S) their
+        perturbed tables with the image surface moved by each one's focus
+        shift, items (n*H*W, 2) the (table, bundle) of every variant and
+        bundle, (v*W + w, h*W + w).  A chunk is `chunk` variants, or as many
+        as fit in 1 GiB of tables, tile rows and `items_per_variant` item
+        rows of `row_bytes` each."""
+        nb = len(self.bundles)
+        W, S = self.nominal.shape[:2]
+        tiles = sum(-(-y.shape[0]//512) for y, _ in self.bundles)
+        step = int(self.chunk) if self.chunk else _variant_chunk(W*S*512, tiles, 2**30, row_bytes,
+                                                                 items_per_variant)
+        if self.compensate == "focus":
+            self.focus = _focus(self.eng, self.fsys, self.nominal, self.params, self.deltas,
+                                self.wavelengths[0], self.rot0, step, self.exact)
+        for v0 in range(0, self.V, step):
+            t = perturbed_tables(self.nominal, self.params, self.deltas[v0:v0 + step])
+            n = len(t)
+            if self.focus is not None:                         # system[-1].distance += shift
+                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
+                                                          self.focus[v0:v0 + n, None])
+            v, b = (a.reshape(-1) for a in np.meshgrid(np.arange(n), np.arange(nb), indexing="ij"))
+            yield v0, t, np.stack([v*W + b % W, b], -1)
+
+    def result(self, out):
+        """`out` with heights, wavelengths, params, deltas and, when
+        compensated, focus"""
+        out.update(heights=np.asarray(self.heights, np.float64),
+                   wavelengths=np.asarray(self.wavelengths, np.float64), params=self.params,
+                   deltas=self.deltas)
+        if self.focus is not None:
+            out["focus"] = self.focus
+        return out
+
+
 def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, nrays=1000,
               distribution="hexapolar", compensate=None, engine=None, exact=False, chunk=None):
     """Spot rms, transmission and centroid of every perturbed lens at every
@@ -353,66 +474,21 @@ def tolerance(system, params, deltas, heights=(0., .707, 1.), wavelengths=None, 
     image, transmitted (V, H, W) the fraction that does, centroid (V, H, W,
     2) relative to the nominal chief ray, moments (V, H, W, 20), focus (V,)
     when compensated, and heights, wavelengths, params, deltas."""
-    from .surface_table import pack_system
-    if compensate not in (None, "focus"):
-        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
-    eng = engine or default_engine()
-    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
-    heights = list(heights)
-    H, W = len(heights), len(wavelengths)
-    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
-    nominal = np.stack([t for t, _, _ in packs])
-    rot0 = packs[0][2]
-    S = nominal.shape[1]
-    params = list(params)
-    deltas = np.asarray(deltas, np.float64)
-    if deltas.ndim == 1:
-        deltas = deltas[None]
-    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
-    V = deltas.shape[0]
-    # System.pupil's result depends on the calls made before it: the focus
-    # bundle is aimed on a copy taken before any
-    fsys = copy.deepcopy(system) if compensate == "focus" else None
-    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    focus = None
-    try:
-        centers = np.array([_chief(eng, nominal[b % W], rot0, y, u, exact)
-                            for b, (y, u) in enumerate(chiefs)])
-        dev = [(y, u, None) for y, u in bundles]
-        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
-        size = W*S*512                                         # device table bytes, FP64
-        step = int(chunk) if chunk else _variant_chunk(size, tiles, 2**30)
-        if step < 1:
-            raise ValueError("chunk must be >= 1")
-        if compensate == "focus":
-            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
-        moments = np.empty((V, H, W, 20))
-        vv, hh, ww = np.meshgrid(np.arange(V), np.arange(H), np.arange(W), indexing="ij")
-        for v0 in range(0, V, step):
-            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+    heights, wavelengths = check_fields(system, heights, wavelengths, compensate, chunk)
+    with VariantMarch(system, params, deltas, heights, wavelengths, nrays, distribution,
+                      compensate, chunk, engine, exact) as r:
+        centers = _centers(r.eng, r.nominal, r.rot0, r.chiefs, exact)
+        H, W, S = r.H, r.W, r.nominal.shape[1]
+        m = np.empty((r.V, H, W, 20))
+        for v0, t, items in r.chunks():
             n = len(t)
-            if focus is not None:                              # system[-1].distance += shift
-                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
-                                                          focus[v0:v0 + n, None])
-            sl = slice(v0*H*W, (v0 + n)*H*W)
-            v, h, w = vv.reshape(-1)[sl] - v0, hh.reshape(-1)[sl], ww.reshape(-1)[sl]
-            items = np.stack([v*W + w, h*W + w], -1)
-            moments[v0:v0 + n] = eng.trace_reduce_many(
-                t.reshape(n*W, S), dev, items, centers[h*W + w], clip=True, rot0=rot0,
+            m[v0:v0 + n] = r.eng.trace_reduce_many(
+                t.reshape(n*W, S), r.dev, items, centers[items[:, 1]], clip=True, rot0=r.rot0,
                 exact=exact).reshape(n, H, W, 20)
-    finally:
-        for y, u in bundles:
-            y.free(), u.free()
-    m = moments
     with np.errstate(all="ignore"):
         out = dict(rms=Engine.rms_finite_from_moments(m), transmitted=m[..., 4]/m[..., 5],
-                   centroid=np.stack([m[..., 1]/m[..., 0], m[..., 2]/m[..., 0]], -1),
-                   moments=m, heights=np.asarray(heights, np.float64),
-                   wavelengths=np.asarray(wavelengths, np.float64), params=params,
-                   deltas=deltas)
-    if focus is not None:
-        out["focus"] = focus
-    return out
+                   centroid=np.stack([m[..., 1]/m[..., 0], m[..., 2]/m[..., 0]], -1), moments=m)
+    return r.result(out)
 
 
 def _otf_targets(targets, shape):
@@ -478,11 +554,7 @@ def tolerance_mtf(system, params, deltas, freqs, heights=(0., .707, 1.), wavelen
     Every argument is checked before any device work."""
     from .engine import OTF_MAX_PLANES
     from .mtf import _check_freqs, _spectral
-    from .surface_table import pack_system
-    if compensate not in (None, "focus"):
-        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
-    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
-    heights = list(heights)
+    heights, wavelengths = check_fields(system, heights, wavelengths, compensate, chunk)
     H, W = len(heights), len(wavelengths)
     nu = _check_freqs(freqs)
     z = np.atleast_1d(np.asarray(defocus, np.float64))
@@ -492,55 +564,22 @@ def tolerance_mtf(system, params, deltas, freqs, heights=(0., .707, 1.), wavelen
     sw = _spectral(spectral_weights, W)
     if targets is not None:
         targets = _otf_targets(targets, (H, 2, F))
-    if chunk is not None and int(chunk) < 1:
-        raise ValueError("chunk must be >= 1")
-    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
-    nominal = np.stack([t for t, _, _ in packs])
-    rot0 = packs[0][2]
-    S = nominal.shape[1]
-    params = list(params)
-    deltas = np.asarray(deltas, np.float64)
-    if deltas.ndim == 1:
-        deltas = deltas[None]
-    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
-    V = deltas.shape[0]
-    eng = engine or default_engine()
-    fsys = copy.deepcopy(system) if compensate == "focus" else None
-    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    focus = None
-    sums = np.empty((V, H, W, K, 2, F), np.complex128)
-    count = np.empty((V, H, W, K), np.int64)
-    try:
+    with VariantMarch(system, params, deltas, heights, wavelengths, nrays, distribution,
+                      compensate, chunk, engine, exact) as r:
         # the chief ray of each height at wavelengths[0], for every wavelength
-        centers = np.array([_chief(eng, nominal[0], rot0, *chiefs[h*W], exact)[:2]
-                            for h in range(H)])
-        dev = [(y, u, None) for y, u in bundles]
-        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
-        step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 8*(4*K*F + K), H*W)
-        if compensate == "focus":
-            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
-        vv, hh, ww = np.meshgrid(np.arange(V), np.arange(H), np.arange(W), indexing="ij")
-        for v0 in range(0, V, step):
-            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+        centers = _centers(r.eng, r.nominal[:1], r.rot0, r.chiefs[::W], exact)[:, :2]
+        S = r.nominal.shape[1]
+        sums = np.empty((r.V, H, W, K, 2, F), np.complex128)
+        count = np.empty((r.V, H, W, K), np.int64)
+        for v0, t, items in r.chunks(8*(4*K*F + K), H*W):
             n = len(t)
-            if focus is not None:                              # system[-1].distance += shift
-                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
-                                                          focus[v0:v0 + n, None])
-            sl = slice(v0*H*W, (v0 + n)*H*W)
-            v, h, w = vv.reshape(-1)[sl] - v0, hh.reshape(-1)[sl], ww.reshape(-1)[sl]
-            s, c = eng.trace_otf_many(t.reshape(n*W, S), dev, np.stack([v*W + w, h*W + w], -1),
-                                      centers[h], z, nu, clip=True, rot0=rot0, exact=exact)
+            s, c = r.eng.trace_otf_many(t.reshape(n*W, S), r.dev, items, centers[items[:, 1]//W],
+                                        z, nu, clip=True, rot0=r.rot0, exact=exact)
             sums[v0:v0 + n] = s.reshape(n, H, W, K, 2, F)
             count[v0:v0 + n] = c.reshape(n, H, W, K)
-    finally:
-        for y, u in bundles:
-            y.free(), u.free()
     out = mtf_tolerance_result(sums, count, sw, targets)
-    out.update(freq=nu, z=z, heights=np.asarray(heights, np.float64),
-               wavelengths=np.asarray(wavelengths, np.float64), params=params, deltas=deltas)
-    if focus is not None:
-        out["focus"] = focus
-    return out
+    out.update(freq=nu, z=z)
+    return r.result(out)
 
 
 # ---- the rms wavefront ------------------------------------------------------
@@ -752,67 +791,22 @@ def tolerance_wavefront(system, params, deltas, heights=(0., .707, 1.), waveleng
     any device work."""
     from .engine import WFE_NSUMS
     from .mtf import _spectral
-    from .surface_table import pack_system
-    if compensate not in (None, "focus"):
-        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
-    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
-    heights = list(heights)
+    heights, wavelengths = check_fields(system, heights, wavelengths, compensate, chunk)
     H, W = len(heights), len(wavelengths)
     sw = _spectral(spectral_weights, W)
     if targets is not None:
         targets = _wfe_targets(targets, H)
-    if chunk is not None and int(chunk) < 1:
-        raise ValueError("chunk must be >= 1")
-    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
-    nominal = np.stack([t for t, _, _ in packs])
-    rot0 = packs[0][2]
-    S = nominal.shape[1]
-    params = list(params)
-    deltas = np.asarray(deltas, np.float64)
-    if deltas.ndim == 1:
-        deltas = deltas[None]
-    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
-    for j, kind in params:
-        if j == S and kind != "distance":
-            raise ValueError("%s of the image surface %d changes only the reference sphere"
-                             % (kind, j))
-    V = deltas.shape[0]
-    eng = engine or default_engine()
-    fsys = copy.deepcopy(system) if compensate == "focus" else None
-    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    ref = _WavefrontRef(system, nominal, wavelengths, chiefs)
-    nb = H*W
-    wl = np.array([l/system.scale for l in wavelengths])
-    focus = None
-    sums = np.empty((V, H, W, WFE_NSUMS))
-    chief = np.empty((V, H, W), bool)
-    try:
-        cdev = ref.upload(eng)
-        dev = [(y, u, None) for y, u in bundles]
-        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
-        step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 160, 3*nb)
-        if compensate == "focus":
-            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
-        for v0 in range(0, V, step):
-            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+    with VariantMarch(system, params, deltas, heights, wavelengths, nrays, distribution,
+                      compensate, chunk, engine, exact, wavefront=True) as r:
+        sums = np.empty((r.V, H, W, WFE_NSUMS))
+        chief = np.empty((r.V, H, W), bool)
+        for v0, t, _ in r.chunks(160, 3*H*W):
             n = len(t)
-            if focus is not None:                              # system[-1].distance += shift
-                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
-                                                          focus[v0:v0 + n, None])
-            march, items, specs, a0, cen, ok = ref.chief(eng, t, rot0, exact)
+            march, items, specs, a0, cen, ok = r.ref.chief(r.eng, t, r.rot0, exact)
             # 4. every ray's residuals about the chief ray's
-            s = eng.trace_opd_many(march, dev, items, specs, a0, cen, clip=True, rot0=rot0,
-                                   exact=exact)
+            s = r.eng.trace_opd_many(march, r.dev, items, specs, a0, cen, clip=True, rot0=r.rot0,
+                                     exact=exact)
             sums[v0:v0 + n] = s.reshape(n, H, W, WFE_NSUMS)
             chief[v0:v0 + n] = ok.reshape(n, H, W)
-    finally:
-        for y, u in bundles:
-            y.free(), u.free()
-        ref.free()
-    Nb = np.array([y.shape[0] for y, _ in bundles], np.float64).reshape(H, W)
-    out = wavefront_tolerance_result(sums, wl, Nb, sw, chief, targets)
-    out.update(heights=np.asarray(heights, np.float64),
-               wavelengths=np.asarray(wavelengths, np.float64), params=params, deltas=deltas)
-    if focus is not None:
-        out["focus"] = focus
-    return out
+    wl = np.array([l/system.scale for l in wavelengths])
+    return r.result(wavefront_tolerance_result(sums, wl, r.counts, sw, chief, targets))

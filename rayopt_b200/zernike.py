@@ -160,82 +160,35 @@ def tolerance_zernike(system, params, deltas, heights=(0., .707, 1.), wavelength
     sums (V, H, W, E) rtx_trace_zernike_many's, focus (V,) when compensated,
     heights, wavelengths, params, deltas.  Every argument is checked before
     any device work."""
-    from .surface_table import pack_system
-    from .tolerance import (_WavefrontRef, _focus, _move_distance, _variant_chunk,
-                            default_engine, launch_bundles, perturbed_tables)
-    import copy
-    if compensate not in (None, "focus"):
-        raise ValueError("compensate must be None or 'focus', got %r" % (compensate,))
+    from .tolerance import VariantMarch, check_fields, perturbed_tables
     order = _check_order(order)
     J = nterms(order)
     E = (J + 1)*(J + 2)//2
-    wavelengths = list(system.wavelengths if wavelengths is None else wavelengths)
-    heights = list(heights)
+    heights, wavelengths = check_fields(system, heights, wavelengths, compensate, chunk)
     H, W = len(heights), len(wavelengths)
-    if H < 1 or W < 1:
-        raise ValueError("need at least one height and one wavelength")
-    if chunk is not None and int(chunk) < 1:
-        raise ValueError("chunk must be >= 1")
-    packs = [pack_system(system, l, 1, None, n0=system.refractive_index(l, 0)) for l in wavelengths]
-    nominal = np.stack([t for t, _, _ in packs])
-    rot0 = packs[0][2]
-    S = nominal.shape[1]
-    params = list(params)
-    deltas = np.asarray(deltas, np.float64)
-    if deltas.ndim == 1:
-        deltas = deltas[None]
-    perturbed_tables(nominal, params, deltas[:0])             # refusals before any device work
-    for j, kind in params:
-        if j == S and kind != "distance":
-            raise ValueError("%s of the image surface %d changes only the reference sphere"
-                             % (kind, j))
-    V = deltas.shape[0]
-    eng = engine or default_engine()
-    fsys = copy.deepcopy(system) if compensate == "focus" else None
-    bundles, chiefs = launch_bundles(system, heights, wavelengths, nrays, distribution, eng)
-    ref = _WavefrontRef(system, nominal, wavelengths, chiefs)
-    nb = H*W
-    wl = np.array([l/system.scale for l in wavelengths])
-    focus = None
-    sums = np.empty((V, H, W, E))
-    chief = np.empty((V, H, W), bool)
-    try:
-        ref.upload(eng)
-        dev = [(y, u, None) for y, u in bundles]
+    with VariantMarch(system, params, deltas, heights, wavelengths, nrays, distribution,
+                      compensate, chunk, engine, exact, wavefront=True) as r:
+        eng, ref, rot0 = r.eng, r.ref, r.rot0
         # rho_b: the nominal lens's largest pupil radius of each bundle (order 0)
-        t = perturbed_tables(nominal, [], np.zeros((1, 0)))
+        t = perturbed_tables(r.nominal, [], np.zeros((1, 0)))
         march, items, specs, a0, cen = ref.chief(eng, t, rot0, exact)[:5]
-        _, r2 = eng.trace_zernike_many(march, dev, items, specs, np.ones(nb), 0, a0, cen,
+        _, r2 = eng.trace_zernike_many(march, r.dev, items, specs, np.ones(H*W), 0, a0, cen,
                                        clip=True, rot0=rot0, exact=exact)
         radius = np.sqrt(r2)
         rho = np.where(radius > 0, radius, 1.)
-        tiles = sum(-(-y.shape[0]//512) for y, _ in bundles)
-        step = int(chunk) if chunk else _variant_chunk(W*S*512, tiles, 2**30, 8*(E + 1), nb)
-        if compensate == "focus":
-            focus = _focus(eng, fsys, nominal, params, deltas, wavelengths[0], rot0, step, exact)
-        for v0 in range(0, V, step):
-            t = perturbed_tables(nominal, params, deltas[v0:v0 + step])
+        sums = np.empty((r.V, H, W, E))
+        chief = np.empty((r.V, H, W), bool)
+        for v0, t, _ in r.chunks(8*(E + 1), H*W):
             n = len(t)
-            if focus is not None:                              # system[-1].distance += shift
-                t["offset"][:, :, -1, 2] = _move_distance(t["offset"][:, :, -1, 2],
-                                                          focus[v0:v0 + n, None])
             march, items, specs, a0, cen, ok = ref.chief(eng, t, rot0, exact)
-            s, _ = eng.trace_zernike_many(march, dev, items, specs, np.tile(rho, n), order, a0,
+            s, _ = eng.trace_zernike_many(march, r.dev, items, specs, np.tile(rho, n), order, a0,
                                           cen, clip=True, rot0=rot0, exact=exact)
             sums[v0:v0 + n] = s.reshape(n, H, W, E)
             chief[v0:v0 + n] = ok.reshape(n, H, W)
-    finally:
-        for y, u in bundles:
-            y.free(), u.free()
-        ref.free()
-    Nb = np.array([y.shape[0] for y, _ in bundles], np.float64).reshape(H, W)
-    out = zernike_result(sums, J, wl, Nb, chief)
-    out.update(radius=np.where(radius > 0, radius, np.nan).reshape(H, W),
-               heights=np.asarray(heights, np.float64),
-               wavelengths=np.asarray(wavelengths, np.float64), params=params, deltas=deltas)
-    if focus is not None:
-        out["focus"] = focus
-    return out
+    wl = np.array([l/system.scale for l in wavelengths])
+    out = zernike_result(sums, J, wl, r.counts, chief)
+    out["radius"] = np.where(radius > 0, radius, np.nan).reshape(H, W)
+    return r.result(out)
 
 
 def zernike_result(sums, J, wl, N, chief=None):

@@ -81,17 +81,14 @@ def host_fit(eng, s0, N, order):
     """the nominal lens's per-ray values of the 9 bundles, fitted on the
     host: (seconds of basis + lstsq per variant, seconds of the downloads,
     largest |c_host - c_device| in waves)"""
-    from rayopt_b200.surface_table import pack_system
-    from rayopt_b200.tolerance import _WavefrontRef, launch_bundles, perturbed_tables
+    from rayopt_b200.tolerance import _nominal, _WavefrontRef, launch_bundles, perturbed_tables
     from rayopt_b200.zernike import nterms, tolerance_zernike, zernike_basis
     J = nterms(order)
     W = len(s0.wavelengths)
     s = copy.deepcopy(s0)
     dev = tolerance_zernike(copy.deepcopy(s0), [], np.zeros((1, 0)), HEIGHTS, nrays=N,
                             order=order, engine=eng)
-    packs = [pack_system(s, l, 1, None, n0=s.refractive_index(l, 0)) for l in s.wavelengths]
-    nominal = np.stack([t for t, _, _ in packs])
-    rot0 = packs[0][2]
+    nominal, rot0 = _nominal(s, s.wavelengths)
     bundles, chiefs = launch_bundles(s, HEIGHTS, s.wavelengths, N, "hexapolar", eng)
     ref = _WavefrontRef(s, nominal, s.wavelengths, chiefs)
     fit_s, dl_s, worst = 0., 0., 0.

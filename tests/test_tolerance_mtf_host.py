@@ -11,18 +11,9 @@ import otf_many_oracle as om
 import ref_shim
 from rayopt_b200.mtf import poly_otf
 from rayopt_b200.tolerance import _variant_chunk, mtf_tolerance_result, tolerance_mtf
+from test_tolerance_driver_host import _NoEngine, _StubSystem
 
 needs_ref = pytest.mark.skipif(not ref_shim.available(), reason="no reference tree staged")
-
-
-class _NoEngine:
-    def __getattr__(self, name):
-        raise AssertionError("device work before the refusal: %s" % name)
-
-
-class _StubSystem:
-    """what the argument refusals read of a System: its wavelengths"""
-    wavelengths = [5.8756e-07, 6.5627e-07, 4.8613e-07]
 
 
 @pytest.mark.parametrize("kw, msg", [

@@ -14,18 +14,9 @@ from rayopt_b200.engine import OPD_DTYPE
 from rayopt_b200.surface_table import pack_system
 from rayopt_b200.tolerance import (perturbed_tables, tolerance_wavefront, wavefront_specs,
                                    wavefront_tolerance_result)
+from test_tolerance_driver_host import _NoEngine, _StubSystem
 
 needs_ref = pytest.mark.skipif(not ref_shim.available(), reason="no reference tree staged")
-
-
-class _NoEngine:
-    def __getattr__(self, name):
-        raise AssertionError("device work before the refusal: %s" % name)
-
-
-class _StubSystem:
-    """what the argument refusals read of a System: its wavelengths"""
-    wavelengths = [5.8756e-07, 6.5627e-07, 4.8613e-07]
 
 
 @pytest.mark.parametrize("kw, msg", [

@@ -10,6 +10,7 @@ import ref_shim
 from rayopt_b200.surface_table import pack_system
 from rayopt_b200.zernike import (noll, nterms, tolerance_zernike, zernike, zernike_basis,
                                  zernike_fit, zernike_result)
+from test_tolerance_driver_host import _NoEngine, _StubSystem
 
 needs_ref = pytest.mark.skipif(not ref_shim.available(), reason="no reference tree staged")
 
@@ -152,16 +153,6 @@ def test_fit_empty_and_lost_chief():
 
 
 # ---- refusals before any device work -----------------------------------------
-class _NoEngine:
-    def __getattr__(self, name):
-        raise AssertionError("device work before the refusal: %s" % name)
-
-
-class _StubSystem:
-    """what the argument refusals read of a System: its wavelengths"""
-    wavelengths = [5.8756e-07, 6.5627e-07, 4.8613e-07]
-
-
 @pytest.mark.parametrize("kw, msg", [
     (dict(order=-1), "order"), (dict(order=9), "order"), (dict(order=2.5), "order"),
     (dict(order=True), "order"), (dict(order="6"), "order"),
